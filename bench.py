@@ -65,6 +65,9 @@ def parse_args():
                     help="en-de workload at N=1: 'realistic' draws sentence lengths from a clipped N(0.6 T, 0.2 T) "
                          "(SURVEY.md 8(d)); the tokens counted are the non-pad target tokens actually in the batches")
     ap.add_argument("--breakdown", action="store_true", help="print the per-entry-point time table")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its losses and a fixed "
+                         "sample of the updated parameters) to DIR/<name>.npy, to compare two builds output for output")
     return ap.parse_args()
 
 
@@ -90,7 +93,7 @@ def workload_config(workload, n_gpus, batch, dropout=True):
                 "optimizer": "LazyAdam beta2 0.98 eps 1e-9, Noam decay (lr 0.2, warmup 4000)",
                 "dropout_keep_prob": 0.9 if dropout else 1.0, "lengths": "fixed (no padding)",
                 "parallelism": "dp{}".format(n_gpus),
-                "l2_between_iters": "parameters + optimizer state (4 x 245 MB) and activations exceed the 126 MB L2"}
+                "l2_between_iters": "parameters + optimizer state (4 x 245 MB) and activations exceed the 50 MB L2"}
     return {"workload": "examples/translation.ini GRU+Bahdanau en-de, synthetic ids",
             "per_gpu_batch": batch, "global_batch": batch * n_gpus, "src_len": ENDE["tx"], "tgt_len": ENDE["ty"],
             "vocab": ENDE["vocab"], "emb": 300, "rnn": 300, "optimizer": "Adam 1e-4, clip 1.0 per tensor, l2 1e-8",
@@ -99,11 +102,10 @@ def workload_config(workload, n_gpus, batch, dropout=True):
                                "shape and replayed; weight gradients are issued on a second stream inside the "
                                "captured backward pass (N>1: the bucketed NCCL all-reduce starts inside the "
                                "backward pass and is captured in the same graph)",
-            "gemm": "tcgen05: kind::f16 for the vocabulary projection and its gradients (fp16 operands, fp32 "
-                    "accumulate), kind::tf32 elsewhere; GRU recurrences on tcgen05 with weights resident in "
-                    "tensor memory",
+            "gemm": "wgmma: fp16 operands for the vocabulary projection and its gradients (fp32 accumulate), "
+                    "tf32 elsewhere; GRU recurrences as persistent cluster kernels in exact fp32",
             "l2_between_iters": "working set per step (0.8 GB fp16 dlogits + 4 x 129 MB parameter buffers) "
-                                "exceeds the 126 MB L2"}
+                                "exceeds the 50 MB L2"}
 
 
 def synthetic_batch(batch, seed, tx=ENDE["tx"], ty=ENDE["ty"], vocab=ENDE["vocab"], realistic=False):
@@ -309,26 +311,42 @@ def measured_peaks():
         return {}
 
 
-def ncu_traffic():
-    """DRAM read+write bytes per launch of the dominant kernels, from this round's committed ncu --set full
-    capture (profiles/r02_traffic.json, written by tools/profile_summary.py); {} when absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-    except Exception:  # pylint: disable=broad-except
-        return {}
+DUMP_PARAM_SAMPLE = 4 << 20      # parameters written by --dump-outputs: 16 MB of float32
+
+
+def dump_outputs(directory, out, arena):
+    """The arrays a caller of the timed step receives - the step's losses (and regularisation sums) - and the
+    parameters the step updated, as DIR/<name>.npy: float64 losses, float32 parameters (a fixed, seeded sample of
+    the flat parameter buffer when it is larger than DUMP_PARAM_SAMPLE elements, in index order; the indices follow
+    from SEED)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    torch.cuda.synchronize()
+
+    def values(x):
+        items = x if isinstance(x, (list, tuple)) else [x]
+        return np.concatenate([torch.as_tensor(v).detach().double().cpu().reshape(-1).numpy() for v in items])
+    np.save(os.path.join(directory, "losses.npy"), values(out["losses"]))
+    if out.get("l1l2") is not None:
+        np.save(os.path.join(directory, "l1l2.npy"), values(out["l1l2"]))
+    flat = arena.params.detach().reshape(-1)
+    if flat.numel() > DUMP_PARAM_SAMPLE:
+        g = torch.Generator().manual_seed(SEED)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(directory, "params_sample.npy"), flat.float().cpu().numpy())
 
 
 def gemm_family_roofline(prof, prof_steps, xent_dims, peaks, total_ms):
     """The dominant kernel is tc_gemm_kernel (csrc/gemm_tc.cu): every dense projection, weight-gradient
     product and the fused vocabulary forward / backward are instances of it.  Algorithmic flops per launch =
     2*M*N*K of the product (DESIGN.md section 3); time = CUDA events around the launches inside the profiled
-    steps.  Instances issuing kind::f16 are rated against the measured bf16 peak, kind::tf32 instances
+    steps.  Instances with fp16 operands are rated against the fp16/bf16 peak, tf32 instances
     cannot exceed half of it (the ceiling is reported too)."""
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
     peak_src = "measured bf16_tflops_sustained (MEASURED_PEAKS.json)" if peaks else \
-        "fallback (B200_PROFILING.md sustained)"
+        "H100 SXM data sheet, dense fp16/bf16 at 700 W"
     m, k, v = xent_dims
-    traffic = ncu_traffic()
     fam_flops = fam_ms = f16_flops = f16_ms = 0.0
     instances = []
     for name, d in prof.items():
@@ -354,19 +372,15 @@ def gemm_family_roofline(prof, prof_steps, xent_dims, peaks, total_ms):
             f16_ms += d["ms"]
         instances.append({"call": name, "launches_per_step": calls // prof_steps,
                           "ms_per_launch": d["ms"] / calls, "tflops": fl / (d["ms"] / calls * 1e-3) / 1e12,
-                          "kind": kind, "traffic": traffic.get(name.split("[")[0])})
+                          "kind": kind})
     if fam_ms <= 0:
         return None
     instances.sort(key=lambda e: -e["ms_per_launch"] * e["launches_per_step"])
     ach = fam_flops / (fam_ms * 1e-3) / 1e12
-    roof = {"kernel": "tc_gemm_kernel (tcgen05; all instances of the step: kind::f16 vocabulary products, "
-                      "kind::tf32 elsewhere)",
+    roof = {"kernel": "tc_gemm_kernel (wgmma; all instances of the step: fp16 vocabulary products, "
+                      "tf32 elsewhere)",
             "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
             "peak_source": peak_src,
-            "traffic": (sum(e["traffic"] for e in instances if e["traffic"]) or None),
-            "traffic_note": "sum of dram__bytes_read+write per launch over the vocabulary instances, from "
-                            "profiles/r02_traffic.json (ncu --set full of this command); null = no capture "
-                            "committed for this build",
             "share_of_step": fam_ms / prof_steps / max(total_ms, 1e-9),
             "instances": instances[:8]}
     if f16_ms > 0:
@@ -377,7 +391,7 @@ def gemm_family_roofline(prof, prof_steps, xent_dims, peaks, total_ms):
 
 
 # ---------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------
 def run_b200(args):
     import bench_models
@@ -424,6 +438,7 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     host_ms = [0.0]
+    last_out = [None]
 
     def timed(step_fn, steps, read_loss):
         barrier()
@@ -433,6 +448,7 @@ def run_b200(args):
         t_host = time.perf_counter()
         for i in range(steps):
             out = step_fn(i)
+            last_out[0] = out
             if read_loss:
                 last = float(out["losses"][0])  # device -> host read of the step's loss
         host_ms[0] = (time.perf_counter() - t_host) * 1e3 / steps   # time the host needs to ENQUEUE a step
@@ -450,6 +466,8 @@ def run_b200(args):
     with (ClockSampler(dev.index or 0) if rank == 0 else contextlib.nullcontext()) as clocks:
         ms_step, _ = timed(step_device_inputs, args.steps, read_loss=False)
     host_enqueue_ms = host_ms[0]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out[0], model.arena)
 
     # per-entry-point device time (CUDA events around every C-ABI call) and the kernel count of a step: these
     # steps issue every launch from Python - a replayed graph contains the same kernel nodes but does not
@@ -573,7 +591,7 @@ def run_b200(args):
 
 
 def ende_parity(model, feed):
-    """The benched engine (tcgen05 fp16/tf32 products, tensor-core GRU, CUDA-graph step) against the fp32
+    """The benched engine (wgmma fp16/tf32 products, cluster GRU, CUDA-graph step) against the fp32
     oracle at the perf dims (H = E = 300, V = 32000, T = 50) on the CPU arm's 16-sentence sample, with O(0.1)
     random parameters so that every activation matters: train loss within 1e-3 (north_star)."""
     from oracle import nm_oracle as O

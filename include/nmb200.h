@@ -1,5 +1,5 @@
 /*
- * nmb200.h -- C ABI of libnmb200.so: the B200 (sm_100a) kernels behind the
+ * nmb200.h -- C ABI of libnmb200.so: the H100 (sm_90a) kernels behind the
  * Neural Monkey encoder-decoder hot path.
  *
  * The reference (ufal/neuralmonkey @ 8b14652) has no FFI boundary: its hot
@@ -35,7 +35,7 @@ extern "C" {
 #define NM_OK 0
 #define NM_E_INVALID (-1)      /* bad argument (null pointer, negative size, ...) */
 #define NM_E_UNSUPPORTED (-2)  /* shape / mode outside what the kernel handles    */
-#define NM_E_NO_DEVICE (-3)    /* no sm_100 device visible                        */
+#define NM_E_NO_DEVICE (-3)    /* no sm_90 device visible                        */
 
 /* activation codes for nm_gemm epilogues and nm_act_bwd */
 #define NM_ACT_NONE 0
@@ -44,9 +44,9 @@ extern "C" {
 #define NM_ACT_SIGMOID 3
 
 /* GEMM backends */
-#define NM_GEMM_AUTO 0  /* tcgen05 when the shape is TMA-addressable, else SIMT */
+#define NM_GEMM_AUTO 0  /* wgmma when the shape is TMA-addressable, else SIMT */
 #define NM_GEMM_SIMT 1  /* fp32 CUDA-core tiles (exact fp32 accumulate)         */
-#define NM_GEMM_TC 2    /* tcgen05 kind::tf32, TMA-staged, TMEM accumulators    */
+#define NM_GEMM_TC 2    /* wgmma tf32, TMA-staged, register accumulators       */
 
 int nm_version(void);
 const char* nm_last_error(void);
@@ -77,11 +77,12 @@ int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K,
             const float* A, int64_t lda, const float* B, int64_t ldb,
             float* C, int64_t ldc, const float* bias, int act, float beta,
             int backend, void* stream);
-/* Tile shape of the tcgen05 products (nm_gemm, nm_gemm_f16*, nm_logits_xent_*): 1 = a CTA pair per 256-row tile
- * (tcgen05.mma.cta_group::2: each SM stages its 128 rows of A and half of the B tile) wherever the shape allows,
- * 0 = one CTA per 128-row tile, -1 = the library's choice per shape (default; NMB200_TC_PAIR presets it). */
+/* Tile shape of the wgmma products (nm_gemm, nm_gemm_f16, nm_logits_xent_*): 1 = a cluster of two CTAs per 256-row
+ * tile wherever the shape allows (B K-major, 128 or 256 columns per tile): each CTA loads half of every B k-block
+ * with a multicast TMA into both; 0 = one CTA per 128-row tile; -1 = the library's choice (default: one CTA;
+ * NMB200_TC_PAIR presets it). */
 int nm_gemm_set_pair_mode(int mode);
-/* 1 if nm_gemm(AUTO) would take the tcgen05 path for this problem. */
+/* 1 if nm_gemm(AUTO) would take the wgmma path for this problem. */
 int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K,
                     int64_t lda, int64_t ldb, int64_t ldc);
 
@@ -154,9 +155,8 @@ int nm_gru_seq_fwd(const float* xproj, const float* Wgh, const float* Wch,
 /* Number of 8-CTA clusters of the persistent GRU kernel that are co-resident on the
  * current device (forward: backward=0).  Diagnostic. */
 int nm_gru_resident_clusters(int backward);
-/* Recurrence engine of nm_gru_seq_fwd/bwd: 0 (default) = tcgen05 tensor cores, recurrent
- * weights resident in tensor memory, TF32 operands with fp32 accumulation; 1 = exact fp32
- * on the CUDA cores (the engine the fp32 parity tests pin against the oracle). */
+/* Recurrence engine of nm_gru_seq_fwd/bwd: 0 (default) or 1; on sm_90a both run the persistent cluster
+ * kernels in exact fp32 (the mode is recorded for callers that set it). */
 int nm_gru_set_mode(int mode);
 /* Diagnostic: 8 int64 device counters receiving the cycles CTA 0 of the forward cluster
  * kernel spends per section (phase 1: load, dot, gates, barrier; phase 2: same). NULL = off. */
@@ -238,7 +238,7 @@ int nm_log_softmax(const float* logits, const float* lse, float* logprobs,
 /* Fused vocabulary projection + loss statistics (K5 without materialising the
  * [M,V] logits): logits = X[M,K].W + b (+ -1e9 at unk_index if >= 0), W stored
  * [K,V] (transW=0) or [V,K] (transW=1: tied embeddings, decoders/autoregressive.py:231-233), on
- * tcgen05; writes lse, xent, argmax as nm_xent_fwd.  part is scratch of
+ * wgmma; writes lse, xent, argmax as nm_xent_fwd.  part is scratch of
  * nm_logits_xent_scratch(M,V) floats (16-byte aligned).  logits_out (may be NULL)
  * additionally receives the [M,V] logits (runtime_logits of the runner API).
  * Returns NM_E_UNSUPPORTED when X/W are not TMA-addressable (rows not multiples
@@ -257,7 +257,7 @@ int nm_logits_xent_bwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
                        float* dlogits, int64_t ldd, int64_t M, int64_t V,
                        int64_t K, void* stream);
 
-/* ---- K5/K6 with fp16 operands (kind::f16), optional path - ops.py uses it with NMB200_XENT16=1 ----
+/* ---- K5/K6 with fp16 operands (fp16 operands), optional path - ops.py uses it with NMB200_XENT16=1 ----
  * Every product is K-major x K-major: X16 [M,K], WT16 [V,K] (the projection matrix transposed),
  * row pitches multiples of 8 elements, bases 16-byte aligned.
  * nm_cast_f16: dst = half(src * row_scale[row]) (row_scale may be NULL) followed by `extra_ones` columns
@@ -275,7 +275,7 @@ int nm_gemm_f16(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, c
                 float beta, int transposed, void* stream);
 /* C[M,N] = alpha_dev[0] * A16^T . B16 (+ C when beta == 1) with both operands stored reduction-major:
  * A16 [K,M] (row pitch lda), B16 [K,N] (row pitch ldb) - the weight-gradient product X^T . dY of the
- * vocabulary projection straight from the row-major fp16 matrices (MN-major tcgen05 operands), no
+ * vocabulary projection straight from the row-major fp16 matrices (MN-major wgmma operands), no
  * transposed copies. */
 int nm_gemm_f16_tn(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16,
                    int64_t ldb, float* C, int64_t ldc, const float* alpha_dev, float beta, void* stream);
@@ -369,7 +369,7 @@ int nm_mha_bwd_drop(const float* q, const float* k, const float* v, const float*
                     float* dk, float* dv, float* de_work, int64_t B, int64_t Tq, int64_t Tk,
                     int64_t heads, int64_t dh, void* stream);
 
-/* The same attention on the tensor cores: every product a batched tcgen05 GEMM over all (sentence, head)
+/* The same attention on the tensor cores: every product a batched wgmma GEMM over all (sentence, head)
  * pairs - P = softmax(mask(Q.K^T/sqrt(dh))) with the softmax in the GEMM epilogue, O = (P*drop).V; backward
  * dS = P*(dO.V^T*drop - rowsum)/sqrt(dh) in the epilogue, dQ = dS.K, dK = dS^T.Q, dV = (P*drop)^T.dO.  TF32
  * operands, fp32 accumulation; q/k/v/out and their gradients keep the [B, T, heads*dh] layout (a head is a
@@ -471,7 +471,7 @@ int nm_attn_decoder_step_set_rows(int rows);
  * (+ -1e9 at unk_index >= 0), lse[m], argmax[m] (first index), and - when symbols_out is given -
  *   symbol = finished_in[m] ? 0 : argmax;  finished_out = finished_in | (symbol == 2);
  *   mask_out = !finished_out;  *unfinished_count += number of rows still unfinished.
- * finished_in/finished_out (u8) may alias.  backend NM_GEMM_AUTO/TC: the tcgen05 GEMM with the
+ * finished_in/finished_out (u8) may alias.  backend NM_GEMM_AUTO/TC: the wgmma GEMM with the
  * softmax-partials epilogue + one combine kernel (`part`: nm_logits_xent_scratch(M,V) floats;
  * logits_out optional).  NM_GEMM_SIMT: exact fp32 CUDA-core GEMM into logits_out (required) + one
  * row kernel.  With targets [M] (gold symbols of this step) xent[m] = (lse - logit[target]) * weights[m]

@@ -1,7 +1,7 @@
-"""In-tree build of libnmb200.so (sm_100a) with plain nvcc.
+"""In-tree build of libnmb200.so (sm_90a, H100) with plain nvcc.
 
-The shared library is written next to this file so that it travels with a
-`gpurun` snapshot; it is git-ignored.  `python -m neuralmonkey_b200.build`
+The shared library is written next to this file (git-ignored), so the package
+is importable from the repository tree.  `python -m neuralmonkey_b200.build`
 rebuilds what is out of date; `--force` rebuilds everything.
 """
 import concurrent.futures
@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(PKG_DIR, "libnmb200.so")
 HEADER = os.path.join(os.path.dirname(PKG_DIR), "include", "nmb200.h")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -56,7 +56,7 @@ def _compile(src: str, force: bool) -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every csrc/*.cu for sm_100a and link libnmb200.so."""
+    """Compile every csrc/*.cu for sm_90a and link libnmb200.so."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     srcs = sources()
     with concurrent.futures.ThreadPoolExecutor(max_workers=8) as pool:
@@ -68,7 +68,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         # link beside the target and rename: a reader (or a snapshot of the tree) never sees half a library
         tmp_path = LIB_PATH + ".tmp.{}".format(os.getpid())
         cmd = [_nvcc(), "-shared", "-o", tmp_path] + objs + [
-            "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+            "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             if os.path.exists(tmp_path):

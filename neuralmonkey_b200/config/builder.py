@@ -6,7 +6,7 @@ A section with `class=dotted.path` becomes the object `path(**other options)`; r
 the section name.  Symbol resolution tries, in order: the literal module path, the `tf.`
 compatibility namespace (neuralmonkey_b200.tf), and `neuralmonkey_b200.<path>` - the place
 the reference looks for `neuralmonkey.<path>` - so unmodified Neural Monkey INI files
-resolve to the B200 implementations.
+resolve to the H100 implementations.
 """
 import importlib
 from argparse import Namespace

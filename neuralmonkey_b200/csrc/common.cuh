@@ -1,4 +1,4 @@
-// Shared helpers for libnmb200 (sm_100a).  Error convention of include/nmb200.h:
+// Shared helpers for libnmb200 (sm_90a).  Error convention of include/nmb200.h:
 // 0 ok, <0 invalid argument, >0 cudaError_t; message via nm_last_error().
 #pragma once
 #include <cuda_runtime.h>
@@ -42,7 +42,7 @@ void count_launches(int64_t n);
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// Number of SMs of the current device (cached per process; 148 on B200).
+// Number of SMs of the current device (cached per process; 132 on an H100 SXM).
 int sm_count();
 
 __device__ __forceinline__ float warp_sum(float v) {

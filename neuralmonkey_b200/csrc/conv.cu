@@ -5,7 +5,7 @@
 // The convolution is an implicit GEMM: M = N*H*W output pixels, N = Cout, K = 9*Cin,
 // A(m, (dy,dx,c)) gathered on the fly from the input (zero outside the image), B = the
 // HWIO filter viewed as [9*Cin, Cout].  Round 1 runs the tile on the CUDA cores in exact
-// fp32; moving it to tcgen05 (TMA im2col) is listed under "what comes next" in DESIGN.md.
+// fp32; a TMA-im2col tensor-core mainloop is listed under "what comes next" in DESIGN.md.
 #include "gemm_simt.cuh"
 
 namespace nm {

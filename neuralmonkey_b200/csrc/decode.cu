@@ -4,7 +4,7 @@
 //   logits = out.W + b (+ -1e9 on <unk>);  symbol = argmax(logits) * !finished;
 //   finished |= (symbol == </s>);  mask = !finished
 //
-// as TWO launches: the tcgen05 GEMM whose epilogue keeps (max, sum exp, argmax) partials per 256-column
+// as TWO launches: the wgmma GEMM whose epilogue keeps (max, sum exp, argmax) partials per 256-column
 // tile (gemm_tc.cu, TC_EPI_XENT_FWD) and a combine kernel that also does the integer bookkeeping, so a
 // decoding step is {nm_attn_decoder_step_fwd, GEMM, combine} with no host-side tensor arithmetic.
 // With the exact-fp32 engine (NM_GEMM_SIMT) the logits are materialised by the CUDA-core GEMM and a

@@ -1,4 +1,4 @@
-// nm_gemm: dense projections.  Dispatches between the tcgen05/TMA kernel
+// nm_gemm: dense projections.  Dispatches between the wgmma/TMA kernel
 // (gemm_tc.cu) and the fp32 CUDA-core tile (gemm_simt.cuh).
 #include "gemm_simt.cuh"
 #include "gemm_tc.h"

@@ -1,23 +1,22 @@
-// tcgen05 GEMM for sm_100a: D[M,N] = op(A)[M,K] . op(B)[K,N], fp32 operands consumed as
-// TF32 (kind::tf32), fp32 accumulation in TMEM.
+// wgmma GEMM for sm_90a: D[M,N] = op(A)[M,K] . op(B)[K,N], fp32 operands consumed as
+// TF32 (or fp16 operands), fp32 accumulation in registers.
 //
-//   * persistent: one CTA per SM walks 128 x BN output tiles (static round-robin);
-//   * warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane) + TMEM allocator,
-//     warps 2..5 = epilogue (TMEM lane quadrant = warp_idx % 4);
-//   * STAGES-deep smem ring of {A 128x32, B BNx32} fp32 tiles in the 128-byte swizzle
-//     (16-byte atoms for K-major operands, 32-byte atoms for MN-major ones),
-//     filled by cp.async.bulk.tensor (OOB rows/cols arrive as zeros: no tail code);
-//   * two TMEM accumulator buffers (2*BN columns) so the epilogue of tile i overlaps
-//     the main loop of tile i+1;
-//   * both operand majors: "K-major" (reduction dim contiguous) and "MN-major"
-//     (reduction dim strided), so forward (X.W), input-gradient (dY.W^T) and
-//     weight-gradient (X^T.dY) products need no transposes in HBM;
+//   * one CTA per 128 x BN output tile (per split-K slice / batched problem);
+//   * warpgroup 0 = producer, warpgroups 1 and 2 = consumers: each issues wgmma.mma_async
+//     m64nBNk8 (tf32) / m64nBNk16 (fp16) for 64 of the tile's rows;
+//   * STAGES-deep smem ring of {A 128 x 128 B, B BN x 128 B} K-major tiles in the 128-byte
+//     swizzle.  K-major operands arrive by cp.async.bulk.tensor (OOB rows / cols as zeros);
+//     wgmma takes TF32 operands K-major only, so MN-major TF32 operands (reduction dim strided)
+//     are loaded by the producer warpgroup's threads and written K-major (transposed, rounded to
+//     TF32) into the same layout; MN-major fp16 operands arrive by TMA as they are stored and
+//     wgmma reads them transposed;
+//   * after the main loop the accumulators go through shared memory (the ring is free by then)
+//     and the epilogue warps read whole 32-column row chunks: one thread = one output row;
 //   * epilogues: dense (bias/activation/accumulate), and the fused vocabulary
 //     cross-entropy forward (online softmax partials + argmax + target logit) and
 //     backward (softmax - onehot), which never materialise fp32 logits twice.
 //
-// Descriptor bit layouts follow the PTX ISA "tcgen05 shared memory descriptor" and
-// "instruction descriptor" tables (as restated in CUTLASS cute/arch/mma_sm100_desc.hpp).
+// Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" of the wgmma section.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -26,28 +25,30 @@
 #include "common.cuh"
 #include "gemm_tc.h"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace nm {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 32;                      // fp32 elements = 128 bytes = one swizzle row
-constexpr int TC_UMMA_K = 8;                   // tf32: 32 bytes per instruction
-constexpr int TC_THREADS = 320;                // TMA warp, MMA warp, 8 epilogue warps
-constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_A_BYTES = TC_BM * TC_BK * 4;  // 16 KB
-constexpr int TC_SMEM_BUDGET = 200 * 1024;
+constexpr int TC_THREADS = 384;                // producer warpgroup, two consumer warpgroups
+constexpr int TC_EPI_WARPS = 8;                // the consumer warps run the epilogue
+constexpr int TC_A_BYTES = TC_BM * 128;        // 16 KB
+constexpr int TC_RING_BUDGET = 192 * 1024;
 
-// CTAS = 2: a CTA pair works on one 256 x BN tile (cta_group::2); each CTA stages BN/2 rows of the B tile
-template <int BN, int CTAS = 1>
+template <int BN>
 struct TcCfg {
-  static constexpr int B_BYTES = (BN / CTAS) * TC_BK * 4;
+  static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
-  static constexpr int STAGES = (TC_SMEM_BUDGET / STAGE_BYTES) > 8 ? 8 : (TC_SMEM_BUDGET / STAGE_BYTES);
-  static constexpr int TMEM_COLS = BN <= 64 ? 128 : (BN <= 128 ? 256 : 512);  // 2*BN rounded to a power of two
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ +
+  static constexpr int STAGES = (TC_RING_BUDGET / STAGE_BYTES) > 4 ? 4 : (TC_RING_BUDGET / STAGE_BYTES);
+  static constexpr int CT_PITCH = BN + 4;      // floats per row of the accumulator tile
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int CT_BYTES = TC_BM * CT_PITCH * 4;
+  static constexpr int UNION_BYTES = RING_BYTES > CT_BYTES ? RING_BYTES : CT_BYTES;
+  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + UNION_BYTES + 256 /*barriers*/ +
                                     TC_EPI_WARPS * 4096 /*per-warp store staging*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "more shared memory than an sm_90 block may have");
 };
-
 // ---------------------------------------------------------------------------
 // epilogue for one 32-column chunk owned by one thread (= one output row).
 // The epilogue runs once per output element, so it is written for instruction count:
@@ -103,7 +104,7 @@ __device__ __forceinline__ void store32(float* __restrict__ c, const float (&x)[
   }
 }
 
-// Coalesced store of a warp's 32x32 chunk.  tcgen05.ld hands every thread one ROW (32 columns),
+// Coalesced store of a warp's 32x32 chunk.  The epilogue hands every thread one ROW (32 columns),
 // so direct stores scatter 16-byte pieces over 32 different cache lines per instruction - the L2
 // request rate, not DRAM, then bounds a kernel that writes a large C (the 1.6 GB dlogits).  Going
 // through a 4 KB per-warp staging tile (XOR-swizzled float4 slots: conflict-free both ways) turns
@@ -381,8 +382,8 @@ __device__ __forceinline__ void epilogue_chunk_dense16(const TcEpilogue& e, cons
 
 // ---------------------------------------------------------------------------
 // TC_EPI_SOFTMAX / TC_EPI_DSOFTMAX: one thread owns one query row of one (sentence, head) problem; the whole
-// row of energies sits in this thread's TMEM lane (N <= BN), so the row reductions need no exchange - the lane
-// is simply read again for every pass (tensor memory is next to the SM).  Mask semantics of the reference
+// row of energies sits in this thread's row of the accumulator tile (N <= BN), so the row reductions need no
+// exchange - the row is simply read again from shared memory for every pass.  Mask semantics of the reference
 // (scaled_dot_product.py:160-206): causal positions are REPLACED by -1e9, padded keys get x*m + (1-m)*(-1e9),
 // both before the softmax; dropout multiplies the softmax output (:208-214).
 //
@@ -413,8 +414,17 @@ __device__ __forceinline__ void load32_coalesced(float* __restrict__ stage, cons
   __syncwarp();
 }
 
+// 32 consecutive accumulators of this thread's row of the tile (16-byte aligned)
+__device__ __forceinline__ void ld_row32(const float* __restrict__ p, float (&x)[32]) {
+#pragma unroll
+  for (int j = 0; j < 32; j += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(p + j);
+    x[j] = v.x; x[j + 1] = v.y; x[j + 2] = v.z; x[j + 3] = v.w;
+  }
+}
+
 template <int MODE>
-__device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch& bt, uint32_t t_row, int r,
+__device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch& bt, const float* crow, int r,
                                               int M, int N, int o, int p, int64_t c_off,
                                               float* __restrict__ stage, int lane) {
   const int nchunks = bt.n_pad >> 5;                 // n_pad is a multiple of 32
@@ -443,7 +453,7 @@ __device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch
     }
   };
   // the rows this tile will read from memory (dropout mask, saved softmax): on their way into L2 while the
-  // tensor-memory passes run
+  // shared-memory passes run
   if (row_ok) {
     if (dbase) asm volatile("prefetch.global.L2 [%0];" ::"l"(dbase + (int64_t)r * N) : "memory");
     if (MODE == TC_EPI_DSOFTMAX) asm volatile("prefetch.global.L2 [%0];" ::"l"(bt.P + c_off + (int64_t)r * e.ldc) : "memory");
@@ -464,21 +474,21 @@ __device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch
     };
     float mx = -INFINITY;
     for (int c = 0; c < nchunks; ++c) {
-      tmem_ld32(t_row + (uint32_t)(c * 32), v);
+      ld_row32(crow + c * 32, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (c * 32 + j < N) mx = fmaxf(mx, energy(v[j], c * 32 + j));
     }
     float sum = 0.f;
     for (int c = 0; c < nchunks; ++c) {
-      tmem_ld32(t_row + (uint32_t)(c * 32), v);
+      ld_row32(crow + c * 32, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (c * 32 + j < N) sum += fast_ex2(energy(v[j], c * 32 + j) - mx);
     }
     const float inv = 1.f / sum;
     for (int c = 0; c < nchunks; ++c) {
-      tmem_ld32(t_row + (uint32_t)(c * 32), v);
+      ld_row32(crow + c * 32, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int col = c * 32 + j;
@@ -498,14 +508,14 @@ __device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch
     float pr[32], d[32];
     float dot = 0.f;
     for (int c = 0; c < nchunks; ++c) {
-      tmem_ld32(t_row + (uint32_t)(c * 32), v);
+      ld_row32(crow + c * 32, v);
       load32_coalesced(stage, pbase, e.ldc, row_base, c * 32, M, pr, lane);   // zero beyond the rows / columns
       load_drop(c * 32, d);
 #pragma unroll
       for (int j = 0; j < 32; ++j) dot = fmaf(v[j] * d[j], pr[j], dot);
     }
     for (int c = 0; c < nchunks; ++c) {
-      tmem_ld32(t_row + (uint32_t)(c * 32), v);
+      ld_row32(crow + c * 32, v);
       load32_coalesced(stage, pbase, e.ldc, row_base, c * 32, M, pr, lane);
       load_drop(c * 32, d);
 #pragma unroll
@@ -521,46 +531,78 @@ __device__ __forceinline__ void attn_epilogue(const TcEpilogue& e, const TcBatch
   }
 }
 
-// smem descriptor fields of an MN-major operand tile (bytes); a kernel argument so a
-// diagnostic run can probe them (NMB200_MN_* environment variables), fixed otherwise.
-struct MnDesc {
-  uint32_t layout, sbo, lbo, kadv;
+// An MN-major operand (reduction dimension strided) as the kernel reads it: [rows, cols] stored with row pitch ld
+// (elements), rows = K, cols = M or N.  Elements outside [rows, cols] read as zeros, as TMA would fill them.
+struct TcOperand {
+  const void* ptr;
+  int64_t rows, cols, ld;
 };
 
-// ESZ = operand element size: 4 = fp32 consumed as TF32 (kind::tf32), 2 = fp16 (kind::f16, K-major
-// operands only).  A k-block is 128 bytes of K either way (32 or 64 elements) and one instruction
-// consumes 32 of them, so the smem ring, the descriptors and the TMEM layout are the same.
-template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ = 4, int CTAS = 1>
+// One k-block of an MN-major operand: R MN rows x 128 bytes of K, written K-major into the 128-byte swizzle
+// (16-byte chunk c of row m at chunk c ^ (m & 7)).  An item is one 32-bit word of a row (one tf32 or two fp16
+// k values); a warp covers 8 rows x 4 words, so the shared-memory stores hit 32 different banks and the loads of
+// one k row are 8 consecutive MN elements.  Called by the 128 threads of the producer warpgroup.
+template <int ESZ, int R>
+__device__ __forceinline__ void load_mn_tile(uint8_t* __restrict__ dst, const TcOperand& op, int64_t k_row0,
+                                             int64_t mn0, int tid) {
+  constexpr int PER = R * 32 / 128;
+#pragma unroll 8
+  for (int j = 0; j < PER; ++j) {
+    const int it = tid + 128 * j;
+    const int b = it & 3, a = (it >> 2) & 7, rest = it >> 5;
+    const int m = (rest % (R / 8)) * 8 + a;
+    const int word = (rest / (R / 8)) * 4 + b;
+    const int64_t col = mn0 + m;
+    const bool col_ok = col < op.cols;
+    uint32_t packed;
+    if constexpr (ESZ == 4) {
+      const int64_t r = k_row0 + word;
+      const float* f = reinterpret_cast<const float*>(op.ptr);
+      packed = to_tf32((col_ok && r < op.rows) ? __ldg(f + r * op.ld + col) : 0.f);
+    } else {
+      const int64_t r = k_row0 + 2 * word;
+      const __half* h = reinterpret_cast<const __half*>(op.ptr);
+      const __half zero = __float2half_rn(0.f);
+      const __half lo = (col_ok && r < op.rows) ? h[r * op.ld + col] : zero;
+      const __half hi = (col_ok && r + 1 < op.rows) ? h[(r + 1) * op.ld + col] : zero;
+      const __half2 v = __halves2half2(lo, hi);
+      packed = *reinterpret_cast<const uint32_t*>(&v);
+    }
+    *reinterpret_cast<uint32_t*>(dst + m * 128 + (((word >> 2) ^ (m & 7)) << 4) + ((word & 3) << 2)) = packed;
+  }
+}
+
+// ESZ = operand element size: 4 = fp32 consumed as TF32, 2 = fp16.  A k-block is 128 bytes of K either way
+// (32 or 64 elements) and one instruction consumes 32 of them, so the smem ring and the descriptors are the same.
+// PAIR: a cluster of two CTAs computes a 256 x BN tile (128 rows each) and shares its B tile: each CTA loads half
+// of every B k-block with a multicast TMA that lands in both CTAs, so a pair pulls B through L2 once instead of
+// twice.  A stage is refilled only when the consumers of BOTH CTAs have released it (their empty barriers count
+// the peer's warps too).  B must be K-major (TMA-loaded).
+template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ = 4, bool PAIR = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               int64_t M, int64_t N, int64_t K, TcEpilogue epi, MnDesc mn, int splits, int kb_per_split,
-               TcExt ext, TcBatch bt) {
-  static_assert(ESZ == 4 || !(A_MN || B_MN) || (BN % 64 == 0), "MN-major fp16 B tiles come in 64-column boxes");
+               TcOperand opa, TcOperand opb, int64_t M, int64_t N, int64_t K, TcEpilogue epi, int splits,
+               int kb_per_split, TcExt ext, TcBatch bt) {
   static_assert(ESZ == 2 || MODE != TC_EPI_XENT_BWD16, "the fp16 epilogue belongs to the fp16 instances");
-  static_assert(CTAS == 1 || CTAS == 2, "one CTA or a CTA pair per tile");
-  static_assert(CTAS == 1 || (BN % 64 == 0), "a pair splits the B tile in two halves of whole swizzle atoms");
+  static_assert(!PAIR || (!B_MN && BN % 16 == 0), "a pair multicasts whole 8-row swizzle atoms of a TMA-loaded B");
   constexpr int BK = 128 / ESZ;                // elements per 128-byte k-block
-  constexpr int BM_T = TC_BM * CTAS;           // rows of one tile (pair: 256, 128 per CTA)
-  constexpr int BN_LOAD = BN / CTAS;           // rows of the B tile this CTA stages
-  using Cfg = TcCfg<BN, CTAS>;
-  // pair mode: rank 0 leads (issues the MMAs, owns the `full` and `tmem_empty` barriers the pair reports to)
-  const uint32_t cta_rank = CTAS == 2 ? cluster_ctarank() : 0u;
-  const bool leader = cta_rank == 0;
-  const int64_t worker = CTAS == 2 ? (int64_t)(blockIdx.x >> 1) : (int64_t)blockIdx.x;
-  const int64_t nworkers = CTAS == 2 ? (int64_t)(gridDim.x >> 1) : (int64_t)gridDim.x;
+  constexpr bool MN16 = ESZ == 2 && A_MN && B_MN;   // fp16, both MN-major: TMA boxes, transposed wgmma operands
+  constexpr bool A_MANUAL = A_MN && !MN16, B_MANUAL = B_MN && !MN16;
+  constexpr bool MANUAL = A_MANUAL || B_MANUAL;      // the producer threads write (some of) the tiles
+  using Cfg = TcCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SW128 tiles: 1 KB aligned
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  // barrier layout (8 B each): full[STAGES] | empty[STAGES] | tmem_full[2] | tmem_empty[2] | tmem ptr
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SW128 tiles: 1 KB aligned
+  const uint32_t smem_base = smem_u32(smem);
+  const uint32_t bar_base = smem_base + Cfg::UNION_BYTES;
+  // barrier layout (8 B each): full[STAGES] | empty[STAGES]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t tiles_m = (M + BM_T - 1) / BM_T;
+  constexpr int TILE_M = PAIR ? 2 * TC_BM : TC_BM;
+  const uint32_t cta_rank = PAIR ? cluster_ctarank() : 0u;
+  const int64_t tiles_m = (M + TILE_M - 1) / TILE_M;
   const int64_t tiles_n = (N + BN - 1) / BN;
   // split-K: the reduction is cut into `splits` slices, each an independent work item whose
   // epilogue adds its partial tile into C with red.global.add (weight-gradient products
@@ -568,267 +610,194 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   // batched: bt.count independent problems of this M x N x K, each a window of the operand tensors (no split-K)
   const bool batched = bt.count > 0;
   const int64_t tiles_per = tiles_m * tiles_n;
-  const int64_t num_tiles = batched ? tiles_per * bt.count : tiles_per * splits;
+  const int64_t tile = PAIR ? (int64_t)(blockIdx.x >> 1) : (int64_t)blockIdx.x;
+  const int64_t tm = tile % tiles_m, tn = (tile / tiles_m) % tiles_n;
   const int num_kb_total = (int)((K + BK - 1) / BK);  // host guarantees no empty split
-
-  if (threadIdx.x == 32) {   // descriptor fetch off the critical path of the first TMA load
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
+  const int split = batched ? 0 : (int)(tile / tiles_per);
+  const int kb_begin = batched ? 0 : split * kb_per_split;
+  const int num_kb = batched ? num_kb_total : min(num_kb_total, kb_begin + kb_per_split) - kb_begin;
+  int prob = 0, prob_o = 0;
+  int32_t a_row = 0, a_col = 0, b_row = 0, b_col = 0;   // this problem's operand windows
+  if (batched) {
+    prob = (int)(tile / tiles_per);
+    prob_o = prob / bt.inner;
+    const int i = prob - prob_o * bt.inner;
+    a_row = prob_o * bt.a_row_outer + i * bt.a_row_inner;
+    a_col = i * bt.a_col_inner;
+    b_row = prob_o * bt.b_row_outer + i * bt.b_row_inner;
+    b_col = i * bt.b_col_inner;
   }
+  const int32_t m0 = (int32_t)(tm * TILE_M) + (int32_t)cta_rank * TC_BM, n0 = (int32_t)(tn * BN);
+
   if (threadIdx.x == 0) {
+    if (!A_MANUAL) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
+    if (!B_MANUAL) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), TC_EPI_WARPS * CTAS);  // one arrive per epilogue warp (of both CTAs)
+      mbar_init(full_bar(s), MANUAL ? 128 : 1);
+      mbar_init(empty_bar(s), TC_EPI_WARPS * (PAIR ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    if constexpr (CTAS == 2) {   // the same warp of both CTAs allocates the pair's columns
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((uint32_t)Cfg::TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((uint32_t)Cfg::TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  if constexpr (CTAS == 2) cluster_sync_all();   // the peer's barriers exist before anything arrives on them
-  tcgen05_fence_after();
-  // Programmatic dependent launch (NMB200_TC_PDL): everything above - barriers, the TMEM allocation - touches no
-  // global memory and may run while the previous kernel of the stream drains; from here on its results are
-  // needed.  Without the launch attribute both instructions do nothing.
+  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers exist before anything arrives on them
+  // Programmatic dependent launch (NMB200_TC_PDL): the barrier set-up above touches no global memory and may run
+  // while the previous kernel of the stream drains; from here on its results are needed.  Without the launch
+  // attribute both instructions do nothing.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t tile = worker; tile < num_tiles; tile += nworkers) {
-        const int32_t m0 = (int32_t)((tile % tiles_m) * BM_T) + (int32_t)cta_rank * TC_BM;
-        const int32_t n0 = (int32_t)(((tile / tiles_m) % tiles_n) * BN) + (int32_t)cta_rank * BN_LOAD;
-        int kb_begin = (int)(tile / tiles_per) * kb_per_split;
-        int kb_end = min(num_kb_total, kb_begin + kb_per_split);
-        int32_t a_row = 0, a_col = 0, b_row = 0, b_col = 0;   // this problem's operand windows
-        if (batched) {
-          const int prob = (int)(tile / tiles_per), o = prob / bt.inner, i = prob - o * bt.inner;
-          a_row = o * bt.a_row_outer + i * bt.a_row_inner;
-          a_col = i * bt.a_col_inner;
-          b_row = o * bt.b_row_outer + i * bt.b_row_inner;
-          b_col = i * bt.b_col_inner;
-          kb_begin = 0;
-          kb_end = num_kb_total;
+  if (warp < 4) {
+    // ===================== producer warpgroup =====================
+    const int ptid = threadIdx.x;
+    for (int kb = 0; kb < num_kb && (MANUAL || ptid == 0); ++kb) {
+      const int s = kb % STAGES;
+      const uint32_t phase = (uint32_t)((kb / STAGES) & 1);
+      if constexpr (PAIR) mbar_wait_cluster(empty_bar(s), phase ^ 1u);   // the peer's releases are cluster-scope
+      else mbar_wait(empty_bar(s), phase ^ 1u);
+      const uint32_t a_dst = smem_base + s * Cfg::STAGE_BYTES;
+      const uint32_t b_dst = a_dst + TC_A_BYTES;
+      const int32_t k0 = (kb_begin + kb) * BK;
+      if (ptid == 0) {
+        constexpr uint32_t TX = (A_MANUAL ? 0u : (uint32_t)TC_A_BYTES) + (B_MANUAL ? 0u : (uint32_t)Cfg::B_BYTES);
+        if (TX) mbar_expect_tx_only(full_bar(s), TX);
+        if constexpr (MN16) {   // boxes {64 MN elements, one k-block of rows}, 8 KB each
+#pragma unroll
+          for (int j = 0; j < TC_BM / 64; ++j)
+            tma_load_2d(a_dst + j * 8192, &map_a, full_bar(s), m0 + a_col + 64 * j, k0 + a_row);
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j)
+            tma_load_2d(b_dst + j * 8192, &map_b, full_bar(s), n0 + b_col + 64 * j, k0 + b_row);
+        } else if (!A_MN) {
+          tma_load_2d(a_dst, &map_a, full_bar(s), k0 + a_col, m0 + a_row);  // box {one k-block, 128 rows}
         }
-        for (int kb = kb_begin; kb < kb_end; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t b_dst = a_dst + TC_A_BYTES;
-          // pair: the leader's barrier counts the bytes of both CTAs
-          if (leader) mbar_expect_tx(full_bar(stage), (uint32_t)(Cfg::STAGE_BYTES * CTAS));
-          const uint32_t full_dst = CTAS == 2 ? mapa_u32(full_bar(stage), 0u) : full_bar(stage);
-          auto tma_load = [&](uint32_t dst, const CUtensorMap* map, int32_t c0, int32_t c1) {
-            if constexpr (CTAS == 2) tma_load_2d_pair(dst, map, full_dst, c0, c1);
-            else tma_load_2d(dst, map, full_dst, c0, c1);
-          };
-          const int32_t k0 = kb * BK;
-          // MN-major tiles arrive as boxes of one 128-byte swizzle row of MN elements (32 fp32 / 64 fp16)
-          // by one k-block of rows: 4 KB (fp32) or 8 KB (fp16) each
-          constexpr int MN_BOX = 128 / ESZ;
-          constexpr int MN_BOX_BYTES = MN_BOX * BK * ESZ;
-          if (!A_MN) {
-            tma_load(a_dst, &map_a, k0 + a_col, m0 + a_row);  // box {one k-block, 128 rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < TC_BM / MN_BOX; ++j)
-              tma_load(a_dst + j * MN_BOX_BYTES, &map_a, m0 + a_col + MN_BOX * j, k0 + a_row);
-          }
-          if (!B_MN) {
-            tma_load(b_dst, &map_b, k0 + b_col, n0 + b_row);  // box {one k-block, BN (pair: BN/2) rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN_LOAD / MN_BOX; ++j)
-              tma_load(b_dst + j * MN_BOX_BYTES, &map_b, n0 + b_col + MN_BOX * j, k0 + b_row);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        if constexpr (PAIR) {   // this CTA's half of the B tile, into both CTAs
+          tma_load_2d_multicast(b_dst + cta_rank * (Cfg::B_BYTES / 2), &map_b, full_bar(s), k0 + b_col,
+                                n0 + b_row + (int32_t)cta_rank * (BN / 2), (uint16_t)3);
+        } else if (!B_MN) {   // (MN16 loaded it above)
+          tma_load_2d(b_dst, &map_b, full_bar(s), k0 + b_col, n0 + b_row);  // box {one k-block, BN rows}
         }
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0 && leader) {
-      // instruction descriptor: c=F32 [4,6)=1, a=TF32 [7,10)=2, b=TF32 [10,13)=2,
-      // a_major bit15, b_major bit16, N>>3 [17,23), M>>4 [24,29)
-      constexpr uint32_t FMT = ESZ == 4 ? 2u : 0u;   // TF32 = 2, F16 = 0
-      const uint32_t idesc = (1u << 4) | (FMT << 7) | (FMT << 10) | ((A_MN ? 1u : 0u) << 15) |
-                             ((B_MN ? 1u : 0u) << 16) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)(BM_T >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int64_t it = 0;
-      for (int64_t tile = worker; tile < num_tiles; tile += nworkers, ++it) {
-        const int acc = (int)(it & 1);
-        const uint32_t acc_phase = (uint32_t)((it >> 1) & 1);
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        const int kb_begin = (int)(tile / tiles_per) * kb_per_split;
-        const int num_kb = batched ? num_kb_total : min(num_kb_total, kb_begin + kb_per_split) - kb_begin;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t b_addr = a_addr + TC_A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TC_BK / TC_UMMA_K; ++k) {
-            // K-major (SWIZZLE_128B): atoms of 8 rows x 128 B, next 8-row group at +1024 B
-            //   (SBO), K step of one instruction (8 tf32) = +32 B inside the swizzled row.
-            // MN-major: tf32 operands whose reduction dim is strided must use the
-            //   128B-swizzle-with-32B-atoms layout (the only MN-major tf32 layout tcgen05
-            //   accepts): atoms of 4 k-rows x 128 B (32 MN elements); next 4-k-row group at
-            //   +512 B (SBO), next 32-element MN atom = next TMA box at +4096 B (LBO);
-            //   K step (8 k-rows) = +1024 B.
-            // MN-major fp16 (kind::f16 takes both majors in the plain 128-byte swizzle): atoms of
-            //   8 k-rows x 128 B (64 MN elements); next 8-k-row group at +1024 B (SBO), next 64-element
-            //   MN atom = next TMA box at +8192 B (LBO); K step of one instruction (16 k-rows) = +2048 B.
-            const uint64_t da = A_MN ? smem_desc(a_addr + k * mn.kadv, mn.lbo, mn.sbo, mn.layout)
-                                     : smem_desc(a_addr + k * 32, 16, 1024, SMEM_LAYOUT_SW128);
-            const uint64_t db = B_MN ? smem_desc(b_addr + k * mn.kadv, mn.lbo, mn.sbo, mn.layout)
-                                     : smem_desc(b_addr + k * 32, 16, 1024, SMEM_LAYOUT_SW128);
-            const uint32_t accum = (kb > 0 || k > 0) ? 1u : 0u;
-            if constexpr (CTAS == 2) {
-              if (ESZ == 4) umma_tf32_pair(d_tmem, da, db, idesc, accum);
-              else umma_f16_pair(d_tmem, da, db, idesc, accum);
-            } else {
-              if (ESZ == 4) umma_tf32(d_tmem, da, db, idesc, accum);
-              else umma_f16(d_tmem, da, db, idesc, accum);
-            }
-          }
-          // frees this smem stage (of both CTAs) when the MMAs retire
-          if constexpr (CTAS == 2) umma_commit_pair(empty_bar(stage), 3);
-          else umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        // accumulator complete -> epilogue (of both CTAs)
-        if constexpr (CTAS == 2) umma_commit_pair(tfull_bar(acc), 3);
-        else umma_commit(tfull_bar(acc));
-      }
+      uint8_t* ring = smem + s * Cfg::STAGE_BYTES;
+      if constexpr (A_MANUAL) load_mn_tile<ESZ, TC_BM>(ring, opa, k0 + a_row, m0 + a_col, ptid);
+      if constexpr (B_MANUAL) load_mn_tile<ESZ, BN>(ring + TC_A_BYTES, opb, k0 + b_row, n0 + b_col, ptid);
+      // the generic-proxy stores above become visible to wgmma (async proxy) before the arrive
+      if constexpr (MANUAL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      mbar_arrive(full_bar(s));
     }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    // Two warps per TMEM lane quadrant (quadrant = warp_idx % 4 is a hardware rule); the
-    // pair splits the tile's 32-column chunks (even / odd), which also gives every SM
-    // sub-partition two epilogue warps to overlap their latencies.
-    const int quad = warp & 3;                // TMEM lanes [32*quad, 32*quad+32)
-    const int half = (warp - 2) >> 2;         // 0: even chunks, 1: odd chunks
-    const bool vec_ok = ((epi.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(epi.C) & 15) == 0);
-    // per-warp staging tile behind the barriers (generic pointer of the 1 KB-aligned window)
-    float* stage = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) +
-                                            STAGES * Cfg::STAGE_BYTES + 256 + (warp - 2) * 4096);
-    const int n32 = (int)N;
-    int64_t it = 0;
-    for (int64_t tile = worker; tile < num_tiles; tile += nworkers, ++it) {
-      const int acc = (int)(it & 1);
-      const uint32_t acc_phase = (uint32_t)((it >> 1) & 1);
-      const int64_t tm = tile % tiles_m, tn = (tile / tiles_m) % tiles_n;
-      const int split = batched ? 0 : (int)(tile / tiles_per);
-      const int64_t row = tm * BM_T + (int64_t)cta_rank * TC_BM + quad * 32 + lane;
-      // batched: this problem's output window
-      int prob = 0, prob_o = 0;
-      int64_t c_off = 0;
-      if (batched) {
-        prob = (int)(tile / tiles_per);
-        prob_o = prob / bt.inner;
-        c_off = (int64_t)prob_o * bt.c_outer + (int64_t)(prob - prob_o * bt.inner) * bt.c_inner;
-      }
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      RowStats st{-INFINITY, 0.f, -INFINITY, 0x7fffffff};
-      int target = -1;
-      float row_lse2 = 0.f, row_w = 0.f;
-      if (MODE != TC_EPI_DENSE && row < M) {
-        if (epi.targets) target = (int)epi.targets[row];
-        if (MODE == TC_EPI_XENT_BWD) {
-          row_lse2 = epi.lse[row] * TC_LOG2E;
-          row_w = (epi.weights ? epi.weights[row] : 1.f) * epi.scale[0];
-        }
-        if (MODE == TC_EPI_XENT_BWD16) {
-          row_lse2 = epi.lse[row] * TC_LOG2E;
-          row_w = epi.weights ? epi.weights[row] : 1.f;
-        }
-      }
-      float factor16 = 1.f;
-      if (ESZ == 2 && MODE == TC_EPI_DENSE) {
-        if (ext.alpha) factor16 = ext.alpha[0];
-        if (ext.row_scale && row < M) factor16 *= ext.row_scale[row];
-      }
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      if constexpr (MODE == TC_EPI_SOFTMAX || MODE == TC_EPI_DSOFTMAX) {
-        // whole rows per thread: the first warp of each lane quadrant does the tile (a handful of columns)
-        if (half == 0) attn_epilogue<MODE>(epi, bt, t_row, (int)row, (int)M, n32, prob_o, prob, c_off, stage, lane);
-      } else {
-      TcEpilogue epi_p = epi;               // this problem's window of C
-      if (batched) epi_p.C += c_off;
-      const TcEpilogue& epi = epi_p;
+  // ===================== consumer warpgroups: main loop =====================
+  const int wg = (warp >> 2) - 1;              // rows [64*wg, 64*wg + 64) of the tile
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int prev_s = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(full_bar(s), (uint32_t)((kb / STAGES) & 1));
+    const uint32_t a_addr = smem_base + s * Cfg::STAGE_BYTES + wg * 64 * 128;   // K-major: 64 rows; MN16: one box
+    const uint32_t b_addr = smem_base + s * Cfg::STAGE_BYTES + TC_A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if constexpr (MN16)
+        Wgmma<BN, 2, true>::mma(acc, gmma_desc_sw128_mn(a_addr + k * 2048), gmma_desc_sw128_mn(b_addr + k * 2048));
+      else
+        Wgmma<BN, ESZ>::mma(acc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32));
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                           // the previous k-block's products are done with their stage
+    wgmma_fence_operands(acc);
+    if (prev_s >= 0 && lane == 0) {
+      mbar_arrive(empty_bar(prev_s));
+      if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(empty_bar(prev_s), cta_rank ^ 1u));   // the peer refills it too
+    }
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operands(acc);
+
+  // ===================== accumulators -> shared memory =====================
+  // the ring is free once both consumer warpgroups are past their last product
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  float* ctile = reinterpret_cast<float*>(smem);
+  {
+    const int wt = threadIdx.x & 127;
+    const int r0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      *reinterpret_cast<float2*>(ctile + r0 * Cfg::CT_PITCH + 8 * i + c0) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(ctile + (r0 + 8) * Cfg::CT_PITCH + 8 * i + c0) =
+          make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  // ===================== epilogue warps =====================
+  // Two warps per 32-row quadrant; the pair splits the tile's 32-column chunks (even / odd).
+  const int ew = warp - 4;
+  const int quad = ew & 3;                     // rows [32*quad, 32*quad+32)
+  const int half = ew >> 2;                    // 0: even chunks, 1: odd chunks
+  const bool vec_ok = ((epi.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(epi.C) & 15) == 0);
+  float* stage = reinterpret_cast<float*>(smem + Cfg::UNION_BYTES + 256) + ew * 1024;   // per-warp staging tile
+  const int n32 = (int)N;
+  const int64_t row = m0 + quad * 32 + lane;
+  const float* crow = ctile + (quad * 32 + lane) * Cfg::CT_PITCH;
+  int64_t c_off = 0;   // batched: this problem's output window
+  if (batched)
+    c_off = (int64_t)prob_o * bt.c_outer + (int64_t)(prob - prob_o * bt.inner) * bt.c_inner;
+  RowStats st{-INFINITY, 0.f, -INFINITY, 0x7fffffff};
+  int target = -1;
+  float row_lse2 = 0.f, row_w = 0.f;
+  if (MODE != TC_EPI_DENSE && row < M) {
+    if (epi.targets) target = (int)epi.targets[row];
+    if (MODE == TC_EPI_XENT_BWD) {
+      row_lse2 = epi.lse[row] * TC_LOG2E;
+      row_w = (epi.weights ? epi.weights[row] : 1.f) * epi.scale[0];
+    }
+    if (MODE == TC_EPI_XENT_BWD16) {
+      row_lse2 = epi.lse[row] * TC_LOG2E;
+      row_w = epi.weights ? epi.weights[row] : 1.f;
+    }
+  }
+  float factor16 = 1.f;
+  if (ESZ == 2 && MODE == TC_EPI_DENSE) {
+    if (ext.alpha) factor16 = ext.alpha[0];
+    if (ext.row_scale && row < M) factor16 *= ext.row_scale[row];
+  }
+  if constexpr (MODE == TC_EPI_SOFTMAX || MODE == TC_EPI_DSOFTMAX) {
+    // whole rows per thread: the first warp of each quadrant does the tile (a handful of columns)
+    if (half == 0) attn_epilogue<MODE>(epi, bt, crow, (int)row, (int)M, n32, prob_o, prob, c_off, stage, lane);
+  } else {
+    TcEpilogue epi_p = epi;               // this problem's window of C
+    if (batched) epi_p.C += c_off;
+    const TcEpilogue& epi = epi_p;
 #pragma unroll 1
-      for (int c = half; c < BN / 32; c += 2) {
-        float v[32];
-        tmem_ld32(t_row + (uint32_t)(c * 32), v);
-        if constexpr (MODE == TC_EPI_XENT_BWD16) {
-          epilogue_chunk_xent_bwd16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, target, row_lse2,
-                                    row_w, stage, lane);
-        } else if constexpr (ESZ == 2 && MODE == TC_EPI_DENSE) {
-          epilogue_chunk_dense16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, factor16, vec_ok,
-                                 stage, lane, st);
-        } else {
+    for (int c = half; c < BN / 32; c += 2) {
+      float v[32];
+      ld_row32(crow + c * 32, v);
+      if constexpr (MODE == TC_EPI_XENT_BWD16) {
+        epilogue_chunk_xent_bwd16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, target, row_lse2,
+                                  row_w, stage, lane);
+      } else if constexpr (ESZ == 2 && MODE == TC_EPI_DENSE) {
+        epilogue_chunk_dense16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, factor16, vec_ok,
+                               stage, lane, st);
+      } else {
         if (MODE == TC_EPI_DENSE && splits > 1)
           epilogue_chunk_atomic(epi, v, row, (int)(tn * BN) + c * 32, M, n32, split == 0,
                                 vec_ok && ((reinterpret_cast<uintptr_t>(epi.bias) & 15) == 0), stage, lane);
         else
           epilogue_chunk<MODE>(epi, v, row, (int)(tn * BN) + c * 32, M, n32, st, target, row_lse2,
                                row_w, vec_ok, stage, lane);
-        }
-      }
-      }
-      if (MODE == TC_EPI_XENT_FWD && row < M)
-        epi.part[(row * tiles_n + tn) * 2 + half] =
-            make_float4(st.mx, st.sum, __int_as_float(st.arg), st.tgt);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CTAS == 2) mbar_arrive_cluster(mapa_u32(tempty_bar(acc), 0u));   // the leader's barrier
-        else mbar_arrive(tempty_bar(acc));
       }
     }
   }
-
-  // teardown: everyone done with TMEM before dealloc
-  tcgen05_fence_before();
-  __syncthreads();
-  if constexpr (CTAS == 2) cluster_sync_all();   // the peer is done with this CTA's barriers and with the pair's TMEM
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if constexpr (CTAS == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                   "r"((uint32_t)Cfg::TMEM_COLS)
-                   : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                   "r"((uint32_t)Cfg::TMEM_COLS)
-                   : "memory");
+  if (MODE == TC_EPI_XENT_FWD && row < M)
+    epi.part[(row * tiles_n + tn) * 2 + half] = make_float4(st.mx, st.sum, __int_as_float(st.arg), st.tgt);
   }
+  // a pair: neither CTA leaves while the other may still arrive on its barriers
+  if constexpr (PAIR) cluster_sync_all();
 }
 
 // ---------------------------------------------------------------------------
@@ -851,49 +820,35 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D fp32 tensor [rows, cols] with row pitch ld (elements); box = {box_cols, box_rows}.
-static uint32_t env_u32(const char* name, uint32_t dflt) {
-  const char* e = getenv(name);
-  return (e && *e) ? (uint32_t)strtoul(e, nullptr, 0) : dflt;
-}
-
-static MnDesc mn_desc_config() {
-  static MnDesc d = {0, 0, 0, 0};
-  static bool init = false;
-  if (!init) {
-    d.layout = env_u32("NMB200_MN_LAYOUT", SMEM_LAYOUT_SW128_32B);
-    d.sbo = env_u32("NMB200_MN_SBO", 512);
-    d.lbo = env_u32("NMB200_MN_LBO", 4096);
-    d.kadv = env_u32("NMB200_MN_KADV", 1024);
-    init = true;
-  }
-  return d;
-}
-
-static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld,
-                    uint32_t box_cols, uint32_t box_rows, bool mn_major) {
-  static int mn_swizzle = -1;  // CUtensorMapSwizzle for MN-major operand tiles
-  if (mn_swizzle < 0) mn_swizzle = (int)env_u32("NMB200_MN_SWIZZLE", (uint32_t)CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+// 2-D fp32 tensor [rows, cols] with row pitch ld (elements), K-major operand tile: box = {one k-block, box_rows},
+// 128-byte swizzle; the TMA unit rounds the fp32 values to TF32 on the way.
+static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, uint32_t box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   NM_REQUIRE(fn != nullptr, NM_E_NO_DEVICE, "tc_gemm: cuTensorMapEncodeTiled not available");
-  static int dtype_mode = -1;  // NMB200_TMA_DTYPE=fp32 keeps raw fp32 bits (MMA truncates)
-  if (dtype_mode < 0) {
-    const char* e = getenv("NMB200_TMA_DTYPE");
-    dtype_mode = (e && strcmp(e, "fp32") == 0) ? 1 : 0;
-  }
   const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   const cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
-  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t box[2] = {(cuuint32_t)TC_BK, box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(map, dtype_mode ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32,
-                        2, const_cast<float*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        mn_major ? (CUtensorMapSwizzle)mn_swizzle : CU_TENSOR_MAP_SWIZZLE_128B,
+  const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   NM_REQUIRE(r == CUDA_SUCCESS, NM_E_INVALID,
              "tc_gemm: cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld", (int)r,
              (long long)rows, (long long)cols, (long long)ld);
   return NM_OK;
+}
+
+static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
+                      uint32_t box_rows);
+
+// One operand: a tensor map when it is K-major, the plain description the producer threads read otherwise.
+static int make_operand(CUtensorMap* map, TcOperand* op, bool mn_major, const void* base, int64_t rows, int64_t cols,
+                        int64_t ld, uint32_t box_rows, int esz) {
+  memset(map, 0, sizeof(*map));
+  *op = TcOperand{base, rows, cols, ld};
+  if (mn_major) return NM_OK;
+  if (esz == 4) return make_map(map, reinterpret_cast<const float*>(base), rows, cols, ld, box_rows);
+  return make_map16(map, base, rows, cols, ld, box_rows);
 }
 
 bool tc_gemm_supported(int transA, int transB, int64_t M, int64_t N, int64_t K, int64_t lda,
@@ -907,87 +862,6 @@ bool tc_gemm_supported(int transA, int transB, int64_t M, int64_t N, int64_t K, 
   return true;
 }
 
-constexpr bool TC_PAIR_DEFAULT = false;   // until the pair instances are verified on the GPU: opt-in only
-// NMB200_TC_PAIR: 0 = never, 1 = wherever the shape allows, unset = the policy of pair_wanted()
-static int g_pair_override = -2;   // nm_gemm_set_pair_mode(); -2 = not set
-static int pair_mode() {
-  static const int mode = [] {
-    const char* e = getenv("NMB200_TC_PAIR");
-    return (e && *e) ? atoi(e) : -1;
-  }();
-  return g_pair_override != -2 ? g_pair_override : mode;
-}
-int tc_gemm_set_pair_mode(int mode) {
-  const int before = pair_mode();
-  g_pair_override = mode;
-  return before;
-}
-
-// A CTA pair per 256 x bn tile (cta_group::2): worth it when the product is bound by the bytes the SMs pull
-// from L2 (large M and N), not for the skinny / split-K shapes whose tiles would no longer fill the chip.
-static bool pair_wanted(int64_t M, int64_t N, int64_t K, int bn, int splits) {
-  (void)K;
-  if (bn != 128 && bn != 256) return false;
-  if (sm_count() < 2 || M < 2 * TC_BM) return false;
-  const int mode = pair_mode();
-  if (mode == 0) return false;
-  if (mode == 1) return true;
-  if (!TC_PAIR_DEFAULT) return false;
-  const int64_t pair_tiles = ceil_div(M, 2 * TC_BM) * ceil_div(N, bn) * splits;
-  return splits == 1 && pair_tiles >= (int64_t)(sm_count() / 2);
-}
-
-template <class Kern, class... Args>
-static int launch_pair_kernel(Kern kern, int smem_bytes, int64_t pair_tiles, cudaStream_t s, Args... args) {
-  const int64_t max_pairs = sm_count() / 2;
-  const int64_t pairs = pair_tiles < max_pairs ? pair_tiles : max_pairs;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * pairs));
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = (size_t)smem_bytes;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args...));
-  NM_LAUNCH_CHECK("tc_gemm_kernel(pair)");
-  return NM_OK;
-}
-
-template <int BN, bool A_MN, bool B_MN, int MODE>
-static int launch_pair(const CUtensorMap& ma, const CUtensorMap& mb, int64_t M, int64_t N, int64_t K,
-                       const TcEpilogue& epi, cudaStream_t s, int splits = 1, int kb_per_split = 0) {
-  using Cfg = TcCfg<BN, 2>;
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE, 4, 2>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  if (kb_per_split <= 0) kb_per_split = (int)ceil_div(K, TC_BK);
-  return launch_pair_kernel(kern, Cfg::SMEM_BYTES, ceil_div(M, 2 * TC_BM) * ceil_div(N, BN) * splits, s, ma, mb, M,
-                            N, K, epi, mn_desc_config(), splits, kb_per_split, TcExt{}, TcBatch{});
-}
-
-template <int BN, int MODE, bool MN = false>
-static int launch_pair16(const CUtensorMap& ma, const CUtensorMap& mb, int64_t M, int64_t N, int64_t K,
-                         const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
-  using Cfg = TcCfg<BN, 2>;
-  auto kern = tc_gemm_kernel<BN, MN, MN, MODE, 2, 2>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  return launch_pair_kernel(kern, Cfg::SMEM_BYTES, ceil_div(M, 2 * TC_BM) * ceil_div(N, BN), s, ma, mb, M, N, K, epi,
-                            MN ? MnDesc{SMEM_LAYOUT_SW128, 1024, 8192, 2048} : MnDesc{0, 0, 0, 0}, 1,
-                            (int)ceil_div(K, 64), ext, TcBatch{});
-}
-
 // NMB200_TC_PDL=1: launch with programmatic stream serialization, so that a kernel's prologue overlaps the tail of
 // its predecessor (the kernel waits with griddepcontrol.wait before it touches global memory)
 static bool pdl_enabled() {
@@ -998,68 +872,67 @@ static bool pdl_enabled() {
   return on;
 }
 
-template <class Kern, class... Args>
-static cudaError_t launch_one(Kern kern, unsigned grid, int smem_bytes, cudaStream_t s, Args... args) {
-  if (!pdl_enabled()) {
-    kern<<<grid, TC_THREADS, smem_bytes, s>>>(args...);
-    return cudaSuccess;
+// one CTA per work item (tile x split-K slice, or tile x batched problem); PAIR: a cluster of two CTAs per
+// 256-row work item
+template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ, bool PAIR = false>
+static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                        int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, int splits, int kb_per_split,
+                        const TcExt& ext, const TcBatch& bt, cudaStream_t s, const char* name) {
+  using Cfg = TcCfg<BN>;
+  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE, ESZ, PAIR>;
+  static bool attr_done = false;
+  if (!attr_done) {
+    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    attr_done = true;
   }
+  const int64_t items = ceil_div(M, PAIR ? 2 * TC_BM : TC_BM) * ceil_div(N, BN) * (bt.count > 0 ? bt.count : splits);
+  NM_REQUIRE(items <= (PAIR ? 0x3fffffffLL : 0x7fffffffLL), NM_E_INVALID, "%s: %lld tiles", name, (long long)items);
+  if (kb_per_split <= 0) kb_per_split = (int)ceil_div(K, 128 / ESZ);
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
+  cfg.gridDim = dim3((unsigned)(PAIR ? 2 * items : items));
   cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = (size_t)smem_bytes;
+  cfg.dynamicSmemBytes = (size_t)Cfg::SMEM_BYTES;
   cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int nattr = 0;
+  if (PAIR) {
+    attr[nattr].id = cudaLaunchAttributeClusterDimension;
+    attr[nattr].val.clusterDim.x = 2;
+    attr[nattr].val.clusterDim.y = 1;
+    attr[nattr].val.clusterDim.z = 1;
+    ++nattr;
+  }
+  if (pdl_enabled()) {
+    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[nattr].val.programmaticStreamSerializationAllowed = 1;
+    ++nattr;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, args...);
-}
-
-template <int BN, bool A_MN, bool B_MN, int MODE>
-static int launch_cfg(const CUtensorMap& ma, const CUtensorMap& mb, int64_t M, int64_t N, int64_t K,
-                      const TcEpilogue& epi, cudaStream_t s, int splits = 1, int kb_per_split = 0) {
-  using Cfg = TcCfg<BN>;
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  const int64_t tiles = ceil_div(M, TC_BM) * ceil_div(N, BN) * splits;
-  const int64_t grid = tiles < sm_count() ? tiles : sm_count();
-  if (kb_per_split <= 0) kb_per_split = (int)ceil_div(K, TC_BK);
-  NM_CUDA_TRY(launch_one(kern, (unsigned)grid, Cfg::SMEM_BYTES, s, ma, mb, M, N, K, epi, mn_desc_config(), splits,
-                         kb_per_split, TcExt{}, TcBatch{}));
-  NM_LAUNCH_CHECK("tc_gemm_kernel");
+  cfg.numAttrs = nattr;
+  NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt));
+  NM_LAUNCH_CHECK(name);
   return NM_OK;
 }
 
-// fp16 operands: no split-K, one wave structure as above.  MN = both operands MN-major (the
-// reduction dimension strided: X^T . dY products), otherwise both K-major.
-template <int BN, int MODE, bool MN = false>
-static int launch_cfg16(const CUtensorMap& ma, const CUtensorMap& mb, int64_t M, int64_t N, int64_t K,
-                        const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
-  using Cfg = TcCfg<BN>;
-  auto kern = tc_gemm_kernel<BN, MN, MN, MODE, 2>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  const int64_t tiles = ceil_div(M, TC_BM) * ceil_div(N, BN);
-  const int64_t grid = tiles < sm_count() ? tiles : sm_count();
-  NM_CUDA_TRY(launch_one(kern, (unsigned)grid, Cfg::SMEM_BYTES, s, ma, mb, M, N, K, epi,
-                         MN ? MnDesc{SMEM_LAYOUT_SW128, 1024, 8192, 2048} : MnDesc{0, 0, 0, 0}, 1,
-                         (int)ceil_div(K, 64), ext, TcBatch{}));
-  NM_LAUNCH_CHECK("tc_gemm_kernel(fp16)");
-  return NM_OK;
+template <int BN, bool A_MN, bool B_MN, int MODE, bool PAIR = false>
+static int launch_cfg(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                      int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, cudaStream_t s, int splits = 1,
+                      int kb_per_split = 0) {
+  return launch_tiles<BN, A_MN, B_MN, MODE, 4, PAIR>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, TcExt{},
+                                               TcBatch{}, s, "tc_gemm_kernel");
 }
 
-// 2-D fp16 tensor [rows, cols] with row pitch ld (elements); box = {64 inner elements, box_rows},
-// 128-byte swizzle.  K-major operand: inner = K, rows = M or N; MN-major: inner = M or N, rows = K
-// (box_rows = 64: one k-block).
+// fp16 operands: no split-K.  MN = both operands MN-major (the reduction dimension strided: X^T . dY products),
+// otherwise both K-major.
+template <int BN, int MODE, bool MN = false, bool PAIR = false>
+static int launch_cfg16(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                        int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
+  return launch_tiles<BN, MN, MN, MODE, 2, PAIR>(ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
+                                           "tc_gemm_kernel(fp16)");
+}
+
+// 2-D fp16 tensor [rows, cols] with row pitch ld (elements), K-major operand tile: box = {64 elements of K,
+// box_rows}, 128-byte swizzle.
 static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
                       uint32_t box_rows) {
   EncodeTiledFn fn = get_encode_fn();
@@ -1078,21 +951,10 @@ static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t 
 }
 
 template <int BN, bool A_MN, bool B_MN, int MODE>
-static int launch_batched(const CUtensorMap& ma, const CUtensorMap& mb, int64_t M, int64_t N, int64_t K,
-                          const TcEpilogue& epi, const TcBatch& bt, cudaStream_t s) {
-  using Cfg = TcCfg<BN>;
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  const int64_t tiles = ceil_div(M, TC_BM) * ceil_div(N, BN) * bt.count;
-  const int64_t grid = tiles < sm_count() ? tiles : sm_count();
-  NM_CUDA_TRY(launch_one(kern, (unsigned)grid, Cfg::SMEM_BYTES, s, ma, mb, M, N, K, epi, mn_desc_config(), 1,
-                         (int)ceil_div(K, TC_BK), TcExt{}, bt));
-  NM_LAUNCH_CHECK("tc_gemm_kernel(batched)");
-  return NM_OK;
+static int launch_batched(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                          int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, const TcBatch& bt, cudaStream_t s) {
+  return launch_tiles<BN, A_MN, B_MN, MODE, 4>(ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s,
+                                               "tc_gemm_kernel(batched)");
 }
 
 int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t a_rows,
@@ -1113,22 +975,43 @@ int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t
              NM_E_UNSUPPORTED, "tc_gemm_batched: attention epilogues take K-major operands and N <= 128 (N=%lld)",
              (long long)N);
   CUtensorMap ma, mb;
-  int rc;
-  if (!a_mn) rc = make_map(&ma, A, a_rows, a_cols, lda, TC_BK, TC_BM, false);
-  else       rc = make_map(&ma, A, a_rows, a_cols, lda, 32, TC_BK, true);
+  TcOperand oa, ob;
+  int rc = make_operand(&ma, &oa, a_mn, A, a_rows, a_cols, lda, TC_BM, 4);
   if (rc) return rc;
-  if (!b_mn) rc = make_map(&mb, B, b_rows, b_cols, ldb, TC_BK, (uint32_t)bn, false);
-  else       rc = make_map(&mb, B, b_rows, b_cols, ldb, 32, TC_BK, true);
+  rc = make_operand(&mb, &ob, b_mn, B, b_rows, b_cols, ldb, (uint32_t)bn, 4);
   if (rc) return rc;
-  if (epi.mode == TC_EPI_SOFTMAX) return launch_batched<128, false, false, TC_EPI_SOFTMAX>(ma, mb, M, N, K, epi, bt, s);
-  if (epi.mode == TC_EPI_DSOFTMAX) return launch_batched<128, false, false, TC_EPI_DSOFTMAX>(ma, mb, M, N, K, epi, bt, s);
+  if (epi.mode == TC_EPI_SOFTMAX)
+    return launch_batched<128, false, false, TC_EPI_SOFTMAX>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+  if (epi.mode == TC_EPI_DSOFTMAX)
+    return launch_batched<128, false, false, TC_EPI_DSOFTMAX>(ma, mb, oa, ob, M, N, K, epi, bt, s);
   NM_REQUIRE(b_mn, NM_E_UNSUPPORTED, "tc_gemm_batched: dense products take an MN-major B operand");
   if (bn == 64) {
-    if (a_mn) return launch_batched<64, true, true, TC_EPI_DENSE>(ma, mb, M, N, K, epi, bt, s);
-    return launch_batched<64, false, true, TC_EPI_DENSE>(ma, mb, M, N, K, epi, bt, s);
+    if (a_mn) return launch_batched<64, true, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+    return launch_batched<64, false, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
   }
-  if (a_mn) return launch_batched<128, true, true, TC_EPI_DENSE>(ma, mb, M, N, K, epi, bt, s);
-  return launch_batched<128, false, true, TC_EPI_DENSE>(ma, mb, M, N, K, epi, bt, s);
+  if (a_mn) return launch_batched<128, true, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+  return launch_batched<128, false, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+}
+
+// CTA pairs (tc_gemm_set_pair_mode): 0 = never, 1 = wherever the shape allows, -1 = the library's policy, which
+// is one CTA per tile (pairs are not measured to be faster on any product of the workloads).  NMB200_TC_PAIR
+// presets the mode.
+static int g_pair_override = -2;   // -2 = not set
+static int pair_mode() {
+  static const int mode = [] {
+    const char* e = getenv("NMB200_TC_PAIR");
+    return (e && *e) ? atoi(e) : -1;
+  }();
+  return g_pair_override != -2 ? g_pair_override : mode;
+}
+int tc_gemm_set_pair_mode(int mode) {
+  const int before = pair_mode();
+  g_pair_override = mode;
+  return before;
+}
+// a pair shares a TMA-loaded (K-major) B tile of 128 or 256 columns between two 128-row halves
+static bool pair_wanted(int64_t M, int bn, bool b_tma) {
+  return pair_mode() == 1 && b_tma && (bn == 128 || bn == 256) && M > TC_BM;
 }
 
 static int pick_bn(int64_t M, int64_t N, int64_t K) {
@@ -1187,51 +1070,40 @@ int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, cons
       }
     }
   }
-  const bool pair = pair_wanted(M, N, K, bn, splits);
   CUtensorMap ma, mb;
-  int rc;
-  if (!a_mn) rc = make_map(&ma, A, M, K, lda, TC_BK, TC_BM, false);
-  else       rc = make_map(&ma, A, K, M, lda, 32, TC_BK, true);
+  TcOperand oa, ob;
+  int rc = a_mn ? make_operand(&ma, &oa, true, A, K, M, lda, TC_BM, 4) : make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 4);
   if (rc) return rc;
-  if (!b_mn) rc = make_map(&mb, B, N, K, ldb, TC_BK, (uint32_t)(pair ? bn / 2 : bn), false);
-  else       rc = make_map(&mb, B, K, N, ldb, 32, TC_BK, true);
+  const bool pair = pair_wanted(M, bn, !b_mn);
+  rc = b_mn ? make_operand(&mb, &ob, true, B, K, N, ldb, (uint32_t)bn, 4)
+            : make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)(pair ? bn / 2 : bn), 4);
   if (rc) return rc;
   if (splits > 1 && epi.beta == 0.f)  // partial sums are added: start from zero
     NM_CUDA_TRY(cudaMemset2DAsync(epi.C, sizeof(float) * epi.ldc, 0, sizeof(float) * N, M, s));
-#define NM_TC_DISPATCH_PAIR(BN_, MODE_)                                                                 \
-  do {                                                                                                 \
-    if (!a_mn && !b_mn) return launch_pair<BN_, false, false, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per); \
-    if (!a_mn && b_mn) return launch_pair<BN_, false, true, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);   \
-    if (a_mn && !b_mn) return launch_pair<BN_, true, false, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);   \
-    return launch_pair<BN_, true, true, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);                       \
+#define NM_TC_DISPATCH(BN_, MODE_)                                                                               \
+  do {                                                                                                           \
+    if (!a_mn && !b_mn) return launch_cfg<BN_, false, false, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per); \
+    if (!a_mn && b_mn) return launch_cfg<BN_, false, true, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);   \
+    if (a_mn && !b_mn) return launch_cfg<BN_, true, false, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);   \
+    return launch_cfg<BN_, true, true, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);                       \
   } while (0)
-  if (pair) {
-    if (epi.mode == TC_EPI_XENT_FWD) {
-      if (b_mn) return launch_pair<256, false, true, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, s);
-      return launch_pair<256, false, false, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, s);
+  if (pair) {   // B K-major
+    if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg<256, false, false, TC_EPI_XENT_FWD, true>(ma, mb, oa, ob, M, N, K, epi, s);
+    if (epi.mode == TC_EPI_XENT_BWD) return launch_cfg<256, false, false, TC_EPI_XENT_BWD, true>(ma, mb, oa, ob, M, N, K, epi, s);
+    if (bn == 128) {
+      if (a_mn) return launch_cfg<128, true, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
+      return launch_cfg<128, false, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
     }
-    if (epi.mode == TC_EPI_XENT_BWD) {
-      if (b_mn) return launch_pair<256, false, true, TC_EPI_XENT_BWD>(ma, mb, M, N, K, epi, s);
-      return launch_pair<256, false, false, TC_EPI_XENT_BWD>(ma, mb, M, N, K, epi, s);
-    }
-    if (bn == 128) NM_TC_DISPATCH_PAIR(128, TC_EPI_DENSE);
-    NM_TC_DISPATCH_PAIR(256, TC_EPI_DENSE);
+    if (a_mn) return launch_cfg<256, true, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
+    return launch_cfg<256, false, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
   }
-#undef NM_TC_DISPATCH_PAIR
-#define NM_TC_DISPATCH(BN_, MODE_)                                                                     \
-  do {                                                                                                 \
-    if (!a_mn && !b_mn) return launch_cfg<BN_, false, false, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);  \
-    if (!a_mn && b_mn) return launch_cfg<BN_, false, true, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);    \
-    if (a_mn && !b_mn) return launch_cfg<BN_, true, false, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);    \
-    return launch_cfg<BN_, true, true, MODE_>(ma, mb, M, N, K, epi, s, splits, kb_per);                        \
-  } while (0)
   if (epi.mode == TC_EPI_XENT_FWD) {  // A is always K-major for the vocabulary projection
-    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, s);
-    return launch_cfg<256, false, false, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, s);
+    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, s);
+    return launch_cfg<256, false, false, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, s);
   }
   if (epi.mode == TC_EPI_XENT_BWD) {
-    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_BWD>(ma, mb, M, N, K, epi, s);
-    return launch_cfg<256, false, false, TC_EPI_XENT_BWD>(ma, mb, M, N, K, epi, s);
+    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_BWD>(ma, mb, oa, ob, M, N, K, epi, s);
+    return launch_cfg<256, false, false, TC_EPI_XENT_BWD>(ma, mb, oa, ob, M, N, K, epi, s);
   }
   if (bn == 64) NM_TC_DISPATCH(64, TC_EPI_DENSE);
   if (bn == 128) NM_TC_DISPATCH(128, TC_EPI_DENSE);
@@ -1249,23 +1121,19 @@ int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t 
                  (reinterpret_cast<uintptr_t>(B) & 15) == 0,
              NM_E_INVALID, "tc_gemm16_mn: fp16 operands need 16-byte aligned bases and row pitches");
   NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16_mn: dense epilogue only");
-  CUtensorMap ma, mb;
+  CUtensorMap ma, mb;   // [K, M] and [K, N] as stored, boxes of 64 columns x one 64-row k-block
   int rc = make_map16(&ma, A, K, M, lda, 64);
   if (rc) return rc;
   rc = make_map16(&mb, B, K, N, ldb, 64);
   if (rc) return rc;
-  // 64-column boxes: BN in {64, 128, 256}
+  const TcOperand oa{A, K, M, lda}, ob{B, K, N, ldb};
   int bn = 256;
   if (N <= 64) bn = 64;
   else if (N <= 128) bn = 128;
   else if (ceil_div(M, TC_BM) * ceil_div(N, 256) < sm_count()) bn = 128;
-  if (pair_wanted(M, N, K, bn, 1)) {
-    if (bn == 128) return launch_pair16<128, TC_EPI_DENSE, true>(ma, mb, M, N, K, epi, ext, s);
-    return launch_pair16<256, TC_EPI_DENSE, true>(ma, mb, M, N, K, epi, ext, s);
-  }
-  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE, true>(ma, mb, M, N, K, epi, ext, s);
-  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE, true>(ma, mb, M, N, K, epi, ext, s);
-  return launch_cfg16<256, TC_EPI_DENSE, true>(ma, mb, M, N, K, epi, ext, s);
+  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  return launch_cfg16<256, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
 }
 
 int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
@@ -1276,26 +1144,28 @@ int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda
                  (reinterpret_cast<uintptr_t>(B) & 15) == 0,
              NM_E_INVALID, "tc_gemm16: fp16 operands need 16-byte aligned bases and row pitches");
   const int bn = (epi.mode == TC_EPI_DENSE) ? pick_bn(M, N, K) : TC_XENT_BN;
-  const bool pair = pair_wanted(M, N, K, bn, 1);
   CUtensorMap ma, mb;
-  int rc = make_map16(&ma, A, M, K, lda, TC_BM);
+  TcOperand oa, ob;
+  int rc = make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 2);
   if (rc) return rc;
-  rc = make_map16(&mb, B, N, K, ldb, (uint32_t)(pair ? bn / 2 : bn));
+  const bool pair = pair_wanted(M, bn, true);
+  rc = make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)(pair ? bn / 2 : bn), 2);
   if (rc) return rc;
   if (pair) {
-    if (epi.mode == TC_EPI_XENT_FWD) return launch_pair16<256, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, ext, s);
-    if (epi.mode == TC_EPI_XENT_BWD16) return launch_pair16<256, TC_EPI_XENT_BWD16>(ma, mb, M, N, K, epi, ext, s);
+    if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg16<256, TC_EPI_XENT_FWD, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+    if (epi.mode == TC_EPI_XENT_BWD16)
+      return launch_cfg16<256, TC_EPI_XENT_BWD16, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
     NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16: unsupported epilogue %d", epi.mode);
-    if (bn == 128) return launch_pair16<128, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
-    return launch_pair16<256, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
+    if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+    return launch_cfg16<256, TC_EPI_DENSE, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
   }
-  if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg16<256, TC_EPI_XENT_FWD>(ma, mb, M, N, K, epi, ext, s);
-  if (epi.mode == TC_EPI_XENT_BWD16) return launch_cfg16<256, TC_EPI_XENT_BWD16>(ma, mb, M, N, K, epi, ext, s);
+  if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg16<256, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  if (epi.mode == TC_EPI_XENT_BWD16) return launch_cfg16<256, TC_EPI_XENT_BWD16>(ma, mb, oa, ob, M, N, K, epi, ext, s);
   NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16: unsupported epilogue %d", epi.mode);
-  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
-  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
-  if (bn == 160) return launch_cfg16<160, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
-  return launch_cfg16<256, TC_EPI_DENSE>(ma, mb, M, N, K, epi, ext, s);
+  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  if (bn == 160) return launch_cfg16<160, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  return launch_cfg16<256, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
 }
 
 }  // namespace nm

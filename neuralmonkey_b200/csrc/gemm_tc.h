@@ -1,4 +1,4 @@
-// Host interface of the tcgen05 GEMM (gemm_tc.cu).
+// Host interface of the wgmma GEMM (gemm_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,7 +33,7 @@ struct TcEpilogue {
                            //   target logit or -inf) per (row, n-tile, epilogue half)
 };
 
-// Extra arguments of the fp16-operand instances (kind::f16, K-major operands only); a separate
+// Extra arguments of the fp16-operand instances; a separate
 // trailing kernel parameter so the TF32 instances keep their parameter layout.
 struct TcExt {
   void* C16;               // xent_bwd16: [M,N] fp16, row pitch ldc16 (elements)
@@ -92,8 +92,9 @@ int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda
 int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                         int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s);
 
-// CTA-pair tiles (cta_group::2, 256 x BN per pair): -1 = the library's policy, 0 = never, 1 = wherever the shape
-// allows.  Returns the previous mode.  Overrides the NMB200_TC_PAIR environment variable.
+// CTA pairs (a cluster of two CTAs per 256 x BN tile sharing a multicast B tile): -1 = the library's policy (one
+// CTA per tile), 0 = never, 1 = wherever the shape allows (B K-major, BN 128 or 256).  Returns the previous mode.
+// Overrides the NMB200_TC_PAIR environment variable.
 int tc_gemm_set_pair_mode(int mode);
 
 }  // namespace nm

@@ -14,7 +14,6 @@
 
 #include "gemm_simt.cuh"
 #include "gru_cluster.cuh"
-#include "gru_tc.cuh"
 
 namespace nm {
 
@@ -143,19 +142,7 @@ bool cluster_path_ok(int64_t H) {
   return forced == 0 && H >= 8 && H <= 320;
 }
 
-// Recurrence engine: 0 = tensor cores (TF32 operands, fp32 accumulate; gru_tc.cuh),
-// 1 = exact fp32 on the CUDA cores (gru_cluster.cuh).  NMB200_GRU=cluster|tc overrides.
-int g_gru_mode = 0;
-bool tc_path_ok(int64_t H) {
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("NMB200_GRU");
-    forced = !e ? 0 : (strcmp(e, "tc") == 0 ? 1 : (strcmp(e, "cluster") == 0 || strcmp(e, "steps") == 0 ? 2 : 0));
-  }
-  if (forced == 2) return false;
-  if (forced == 0 && g_gru_mode != 0) return false;
-  return H >= 1 && H <= GT_MAX_UPC * GT_CLUSTER;
-}
+int g_gru_mode = 0;   // nm_gru_set_mode(): recorded; every mode runs the cluster engine on sm_90a
 
 struct ClusterPlan {
   int Bc, nclusters, ch;
@@ -236,74 +223,6 @@ int launch_cluster(Kern kern, const Args& args, const ClusterPlan& p, cudaStream
   return NM_OK;
 }
 
-struct TcPlan {
-  int Bc, nclusters;
-  size_t smem;
-};
-
-template <class Kern>
-int tc_resident_clusters(Kern kern, size_t smem) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(GT_CLUSTER * 64);
-  cfg.blockDim = dim3(GT_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = GT_CLUSTER;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  int n = 0;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-      cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n < 1) {
-    cudaGetLastError();
-    n = sm_count() / GT_CLUSTER / 2;
-  }
-  return n;
-}
-
-template <int ESZ, class Kern>
-TcPlan plan_tc(Kern kern, int64_t B, int64_t H, int sm_budget, int ntiles, int* cache) {
-  const GtGeom<ESZ> geo((int)H);
-  const GtSmem lay(geo.tile_bytes, ntiles);
-  TcPlan p;
-  p.smem = (size_t)lay.total;
-  if (*cache == 0)
-    *cache = tc_resident_clusters(kern, (size_t)GtSmem(GtGeom<ESZ>(GT_MAX_UPC * GT_CLUSTER).tile_bytes, ntiles).total);
-  int max_clusters = *cache;
-  if (sm_budget > 0 && sm_budget / GT_CLUSTER < max_clusters) max_clusters = sm_budget / GT_CLUSTER;
-  if (max_clusters < 1) max_clusters = 1;
-  int Bc = (int)((B + max_clusters - 1) / max_clusters);
-  if (Bc > GT_NB) Bc = GT_NB;  // more sentences than one wave holds: clusters queue up
-  p.Bc = Bc;
-  p.nclusters = (int)((B + Bc - 1) / Bc);
-  return p;
-}
-
-// One sequence (args2 == nullptr) or two co-resident ones: clusters [0, nclusters) work on `args`,
-// [nclusters, 2*nclusters) on `*args2`.
-template <class Args, class Kern>
-int launch_tc(Kern kern, const Args& args, const TcPlan& p, cudaStream_t s, const char* name,
-              const Args* args2 = nullptr) {
-  NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(p.nclusters * GT_CLUSTER * (args2 ? 2 : 1)));
-  cfg.blockDim = dim3(GT_THREADS);
-  cfg.dynamicSmemBytes = p.smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = GT_CLUSTER;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args, args2 ? *args2 : args, p.nclusters));
-  NM_LAUNCH_CHECK(name);
-  return NM_OK;
-}
-
 #define NM_GC_DISPATCH(KERN, args, plan, s, name)                   \
   switch ((plan).ch) {                                              \
     case 1: return launch_cluster(KERN<1>, args, plan, s, name);    \
@@ -340,14 +259,6 @@ int nm_gru_seq_fwd(const float* xproj, const float* Wgh, const float* Wch, const
   NM_REQUIRE(B > 0 && T > 0 && H > 0, NM_E_INVALID, "nm_gru_seq_fwd: bad sizes B=%lld T=%lld H=%lld",
              (long long)B, (long long)T, (long long)H);
   cudaStream_t s = (cudaStream_t)stream;
-  if (tc_path_ok(H) && T * H < (1 << 24)) {
-    static int resident = 0;
-    GtFwdArgs a{xproj, Wgh, Wch, h0, lengths, drop_mask, states, raw_states, final_state, gates,
-                hprev, rh, (int)B, (int)T, (int)H, 0, reverse, g_gru_prof};
-    const TcPlan p = plan_tc<2>(gru_seq_fwd_tc_kernel, B, H, sm_budget, 2, &resident);
-    a.Bc = p.Bc;
-    return launch_tc(gru_seq_fwd_tc_kernel, a, p, s, "nm_gru_seq_fwd(tc)");
-  }
   if (cluster_path_ok(H)) {
     GcFwdArgs a{xproj, Wgh, Wch, h0, lengths, drop_mask, states, raw_states, final_state, gates,
                 hprev, rh, (int)B, (int)T, (int)H, 0, reverse, g_gru_prof};
@@ -388,14 +299,6 @@ int nm_gru_seq_bwd(const float* Wgh, const float* Wch, const int32_t* lengths,
              "nm_gru_seq_bwd: null pointer");
   NM_REQUIRE(B > 0 && T > 0 && H > 0, NM_E_INVALID, "nm_gru_seq_bwd: bad sizes");
   cudaStream_t s = (cudaStream_t)stream;
-  if (tc_path_ok(H) && T * H < (1 << 24)) {
-    static int resident = 0;
-    GtBwdArgs a{Wgh, Wch, lengths, drop_mask, gates, hprev, dstates, draw, dfinal, dxproj, dh0,
-                (int)B, (int)T, (int)H, 0, reverse};
-    const TcPlan p = plan_tc<4>(gru_seq_bwd_tc_kernel, B, H, sm_budget, 3, &resident);
-    a.Bc = p.Bc;
-    return launch_tc(gru_seq_bwd_tc_kernel, a, p, s, "nm_gru_seq_bwd(tc)");
-  }
   if (cluster_path_ok(H)) {
     GcBwdArgs a{Wgh, Wch, lengths, drop_mask, gates, hprev, dstates, draw, dfinal, dxproj, dh0,
                 (int)B, (int)T, (int)H, 0, reverse};
@@ -432,7 +335,7 @@ int nm_gru_seq_bwd(const float* Wgh, const float* Wch, const int32_t* lengths,
 }
 
 
-/* ---- both directions of a bidirectional layer in ONE launch (tensor-core engine) ------------------ */
+/* ---- both directions of a bidirectional layer: one sequence after the other ------------------------ */
 int nm_gru_seq_fwd_pair(const float* xproj_a, const float* Wgh_a, const float* Wch_a, int reverse_a,
                         float* states_a, float* final_a, float* gates_a, float* hprev_a, float* rh_a,
                         const float* xproj_b, const float* Wgh_b, const float* Wch_b, int reverse_b,
@@ -442,21 +345,6 @@ int nm_gru_seq_fwd_pair(const float* xproj_a, const float* Wgh_a, const float* W
                  Wgh_b && Wch_b && states_b && final_b && gates_b && hprev_b && rh_b,
              NM_E_INVALID, "nm_gru_seq_fwd_pair: null pointer");
   NM_REQUIRE(B > 0 && T > 0 && H > 0, NM_E_INVALID, "nm_gru_seq_fwd_pair: bad sizes");
-  if (tc_path_ok(H) && T * H < (1 << 24)) {
-    static int resident = 0;
-    plan_tc<2>(gru_seq_fwd_tc_kernel, B, H, 0, 2, &resident);                 // fills `resident`
-    const int half_budget = (resident / 2) * GT_CLUSTER;
-    if (half_budget >= GT_CLUSTER) {
-      const TcPlan p = plan_tc<2>(gru_seq_fwd_tc_kernel, B, H, half_budget, 2, &resident);
-      if (2 * p.nclusters <= resident) {                                        // both sequences co-resident
-        GtFwdArgs a{xproj_a, Wgh_a, Wch_a, nullptr, lengths, nullptr, states_a, nullptr, final_a, gates_a,
-                    hprev_a, rh_a, (int)B, (int)T, (int)H, p.Bc, reverse_a, nullptr};
-        GtFwdArgs b{xproj_b, Wgh_b, Wch_b, nullptr, lengths, nullptr, states_b, nullptr, final_b, gates_b,
-                    hprev_b, rh_b, (int)B, (int)T, (int)H, p.Bc, reverse_b, nullptr};
-        return launch_tc(gru_seq_fwd_tc_kernel, a, p, (cudaStream_t)stream, "nm_gru_seq_fwd_pair(tc)", &b);
-      }
-    }
-  }
   int rc = nm_gru_seq_fwd(xproj_a, Wgh_a, Wch_a, nullptr, lengths, nullptr, reverse_a, states_a, nullptr, final_a,
                           gates_a, hprev_a, rh_a, B, T, H, 0, stream);
   if (rc) return rc;
@@ -473,21 +361,6 @@ int nm_gru_seq_bwd_pair(const float* Wgh_a, const float* Wch_a, int reverse_a, c
                  dxproj_b && work,
              NM_E_INVALID, "nm_gru_seq_bwd_pair: null pointer");
   NM_REQUIRE(B > 0 && T > 0 && H > 0, NM_E_INVALID, "nm_gru_seq_bwd_pair: bad sizes");
-  if (tc_path_ok(H) && T * H < (1 << 24)) {
-    static int resident = 0;
-    plan_tc<4>(gru_seq_bwd_tc_kernel, B, H, 0, 3, &resident);
-    const int half_budget = (resident / 2) * GT_CLUSTER;
-    if (half_budget >= GT_CLUSTER) {
-      const TcPlan p = plan_tc<4>(gru_seq_bwd_tc_kernel, B, H, half_budget, 3, &resident);
-      if (2 * p.nclusters <= resident) {
-        GtBwdArgs a{Wgh_a, Wch_a, lengths, nullptr, gates_a, hprev_a, dstates_a, nullptr, dfinal_a, dxproj_a,
-                    nullptr, (int)B, (int)T, (int)H, p.Bc, reverse_a};
-        GtBwdArgs b{Wgh_b, Wch_b, lengths, nullptr, gates_b, hprev_b, dstates_b, nullptr, dfinal_b, dxproj_b,
-                    nullptr, (int)B, (int)T, (int)H, p.Bc, reverse_b};
-        return launch_tc(gru_seq_bwd_tc_kernel, a, p, (cudaStream_t)stream, "nm_gru_seq_bwd_pair(tc)", &b);
-      }
-    }
-  }
   int rc = nm_gru_seq_bwd(Wgh_a, Wch_a, lengths, nullptr, reverse_a, gates_a, hprev_a, dstates_a, nullptr, dfinal_a,
                           dxproj_a, nullptr, work, B, T, H, 0, stream);
   if (rc) return rc;

@@ -1,4 +1,4 @@
-// Persistent GRU sequence kernels for thread-block clusters (sm_100a).
+// Persistent GRU sequence kernels for thread-block clusters (sm_90a).
 //
 // One launch runs the whole time loop.  A cluster of 8 CTAs owns a slice of the batch
 // (Bc sentences); inside it, CTA r owns hidden units [r*UW, (r+1)*UW), UW = ceil(H/8).

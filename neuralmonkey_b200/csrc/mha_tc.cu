@@ -1,5 +1,5 @@
 // K8 on the tensor cores: multi-head scaled dot-product attention (attention/scaled_dot_product.py:160-214 of the
-// reference) as BATCHED tcgen05 products - one 128 x N tile per (sentence, head), all heads of all sentences in
+// reference) as BATCHED wgmma products - one 128 x N tile per (sentence, head), all heads of all sentences in
 // one launch of the persistent GEMM kernel (gemm_tc.cu, TcBatch):
 //
 //   forward    P  = softmax(mask(Q K^T / sqrt(dh)))        K-major x K-major, softmax in the epilogue (TC_EPI_SOFTMAX)

@@ -1,5 +1,5 @@
-// PTX wrappers shared by the tcgen05 kernels (gemm_tc.cu, gru_tc.cuh): mbarrier, TMA,
-// tcgen05 alloc/mma/ld/st/commit, shared-memory matrix descriptors, cluster (DSMEM) access.
+// PTX wrappers shared by the sm_90a kernels (gemm_tc.cu, decoder_step.cu): mbarrier, TMA,
+// wgmma fences and shared-memory matrix descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -45,160 +45,32 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&r)[32]) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]),
-        "=r"(u[7]), "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]),
-        "=r"(u[14]), "=r"(u[15]), "=r"(u[16]), "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]),
-        "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]), "=r"(u[25]), "=r"(u[26]), "=r"(u[27]),
-        "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle, version 1 (Blackwell).
-// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version | [61,64) layout
-constexpr uint32_t SMEM_LAYOUT_SW128 = 2;       // 128-byte swizzle, 16-byte atoms
-constexpr uint32_t SMEM_LAYOUT_SW128_32B = 1;   // 128-byte swizzle, 32-byte atoms
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t layout) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
-}
-
-
-// ---- TMEM stores, A-operand-in-TMEM MMA, cluster / distributed shared memory --------------
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&u)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0],"
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16,"
-      " %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3]), "r"(u[4]), "r"(u[5]), "r"(u[6]), "r"(u[7]),
-      "r"(u[8]), "r"(u[9]), "r"(u[10]), "r"(u[11]), "r"(u[12]), "r"(u[13]), "r"(u[14]), "r"(u[15]),
-      "r"(u[16]), "r"(u[17]), "r"(u[18]), "r"(u[19]), "r"(u[20]), "r"(u[21]), "r"(u[22]),
-      "r"(u[23]), "r"(u[24]), "r"(u[25]), "r"(u[26]), "r"(u[27]), "r"(u[28]), "r"(u[29]),
-      "r"(u[30]), "r"(u[31])
-      : "memory");
-}
-// 16 consecutive 32-bit columns of this thread's TMEM lane (no wait: pair with tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float (&r)[16]) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]),
-        "=r"(u[7]), "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]),
-        "=r"(u[14]), "=r"(u[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// fast transcendental forms for the tensor-core recurrence (ex2.approx + rcp.approx: ~1e-7 rel)
-__device__ __forceinline__ float fast_sigmoid(float x) {
-  return __fdividef(1.f, 1.f + __expf(-x));
-}
-__device__ __forceinline__ float fast_tanh_exp(float x) {
-  // 1 - 2/(1+e^{2x}); saturates cleanly for |x| large
-  return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x));
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem desc]   (A: 128 lanes x K 32-bit columns)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 (fp16 / bf16 operands, fp32 accumulate), A operand in tensor memory: one 32-bit TMEM
-// column holds two consecutive K elements
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// expect `bytes` more transaction bytes on the barrier without arriving on it
+__device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return u;
 }
+
+// ---- clusters: CTA pairs sharing the B tile (multicast TMA, remote barrier arrivals) ------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t cta_rank) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
   return r;
 }
-__device__ __forceinline__ void st_cluster_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c,
-                                              uint32_t d) {
-  asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
-               "r"(d)
-               : "memory");
-}
-// Asynchronous 16-byte store into (possibly remote) cluster shared memory; the bytes are counted
-// on the mbarrier at `mbar` (a shared::cluster address in the same CTA as `addr`).
-__device__ __forceinline__ void st_async_v4(uint32_t addr, uint32_t mbar, uint32_t a, uint32_t b,
-                                            uint32_t c, uint32_t d) {
-  asm volatile(
-      "st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(addr),
-      "r"(a), "r"(b), "r"(c), "r"(d), "r"(mbar)
-      : "memory");
-}
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr)
-               : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
   asm volatile(
@@ -213,58 +85,46 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
       "r"(parity)
       : "memory");
 }
-// ---- CTA pairs (cta_group::2): two SMs of one TPC execute one 256-row MMA.  Each CTA stages its own 128 rows
-// of A and HALF of the B tile, so the bytes a CTA pulls through the L2 fabric per flop drop by a third to a half;
-// the leader (cluster rank 0) issues the MMAs, both CTAs' TMA loads report to the LEADER's mbarrier, and the
-// leader's commits arrive at the barriers of both CTAs.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// `bar` is a shared::cluster address (mapa of the leader's barrier)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar,
-                                                 int32_t c0, int32_t c1) {
+// the box lands at the same CTA-relative offset in every CTA of `mask`, and its bytes are counted on the barrier at
+// the same offset in each of them
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int32_t c0,
+                                                      int32_t c1, uint16_t mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-// arrive (when the MMAs issued so far retire) on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
+
+// ---- wgmma (warpgroup MMA) ---------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_tf32_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// keeps the compiler from moving accesses of accumulator registers across a wgmma wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+
+// Shared-memory matrix descriptor of a K-major operand tile in the 128-byte swizzle (rows of 128 bytes,
+// 8-row atoms of 1 KB, tile base 1 KB aligned): start address >> 4 at [0,14), leading byte offset (unused
+// by swizzled K-major layouts, 1) at [16,30), stride byte offset 1024 >> 4 at [32,46), layout 1 = 128B
+// swizzle at [62,64).  Advancing `addr` by 32 bytes steps K by one instruction (8 tf32 / 16 fp16).
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t addr) {
+  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async;" ::: "memory");
+
+// The same for an MN-major 16-bit operand tile built from TMA boxes of 64 MN elements (128 B) x 64 k-rows in the
+// 128-byte swizzle: 8-k-row atoms of 1 KB along K (stride byte offset 1024), the next 64 MN elements one 8 KB
+// box further (leading byte offset 8192).  Advancing `addr` by 2048 bytes steps K by one instruction (16 rows).
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t addr) {
+  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
 
 }  // namespace nm

@@ -5,7 +5,7 @@
 // written once (1.6 GB at the bench shape) and read about three times.  Here it is stored as fp16,
 // UNNORMALISED ((softmax - onehot) * mask, values in [-1, 1]: fp16 then has TF32's 10 mantissa bits;
 // tools/fp16_dlogits_study.py), once row-major (for dX) and once transposed (for dW), so that every
-// product is a K-major x K-major kind::f16 GEMM:
+// product is a K-major x K-major fp16 wgmma GEMM:
 //     logits  = X16 [M,K]   . WT16 [V,K]^T          (forward and the recompute of the backward)
 //     dX      = dl16 [M,V]  . W16  [K,V]^T           * row_scale[m]
 //     dW^T    = dlT16 [V,M] . XT16 [K+1,M]^T         * alpha, stored transposed into dW (+ db row)
@@ -76,7 +76,8 @@ int nm_cast_f16(const float* src, int64_t ld_src, void* dst, int64_t ld_dst, int
     NM_REQUIRE(extra_ones >= 0 && ld_dst >= cols + extra_ones, NM_E_INVALID, "nm_cast_f16: bad destination pitch");
     const int64_t total = rows * ld_dst;
     const int64_t blocks = ceil_div(total, 256 * 4);
-    cast_f16_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, s>>>(
+    const int64_t cap = (int64_t)sm_count() * 16;   // grid-stride: 16 blocks of 256 threads per SM
+    cast_f16_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, s>>>(
         src, ld_src, reinterpret_cast<__half*>(dst), ld_dst, rows, cols, row_scale, extra_ones);
   } else {
     NM_REQUIRE(ld_dst >= rows && extra_ones >= 0, NM_E_INVALID, "nm_cast_f16: bad destination pitch");

@@ -5,7 +5,7 @@ decoders/autoregressive.py:442-562, wrapped by decoders/beam_search_decoder.py:3
 of libnmb200 and no torch arithmetic:
 
     nm_attn_decoder_step_fwd   embedding row, GRU cell, query projection, Bahdanau attention, deep output
-    nm_decode_logits_step      tcgen05 vocabulary GEMM with softmax partials  +  combine kernel doing the
+    nm_decode_logits_step      wgmma vocabulary GEMM with softmax partials  +  combine kernel doing the
                                argmax / `* unfinished` / `finished |= </s>` bookkeeping
 
 (beam search adds the two kernels of nm_beam_step_logits, which reads the logits and their logsumexp

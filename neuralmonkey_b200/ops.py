@@ -19,7 +19,7 @@ _GEMM_BACKEND = lib.GEMM_AUTO
 
 
 def set_gemm_backend(name: str) -> None:
-    """'auto' (tcgen05 when TMA-addressable), 'simt' (exact fp32) or 'tc'."""
+    """'auto' (wgmma tensor cores when TMA-addressable), 'simt' (exact fp32) or 'tc'."""
     global _GEMM_BACKEND
     _GEMM_BACKEND = {"auto": lib.GEMM_AUTO, "simt": lib.GEMM_SIMT, "tc": lib.GEMM_TC}[name]
     # the GRU recurrence follows: exact fp32 engine with 'simt', tensor cores otherwise
@@ -93,7 +93,7 @@ def weight_grad_stream(enable: bool) -> None:
     _wg["open"] = bool(enable)
 
 
-_WGRAD_STREAM_DEFAULT = "1"    # Transformer step 12.75 -> 12.25 ms, en-de unchanged; NMB200_WGRAD_STREAM=0 shuts it
+_WGRAD_STREAM_DEFAULT = "1"    # weight gradients on a second stream; NMB200_WGRAD_STREAM=0 shuts it
 
 
 def join_weight_grads() -> None:
@@ -711,8 +711,8 @@ class _LogitsXent16(torch.autograd.Function):
         P16    = half((softmax - onehot) * mask) [M,V]      written ONCE, row-major (0.8 GB at the bench shape,
                                                             against 1.6 GB fp32 written once and read twice)
         dX     = P16 . W16 [K,V]^T * upstream[m]            K-major x K-major
-        dW,db  = [X * u, u]16^T . P16 * max|upstream|       both operands MN-major (tcgen05 takes either
-                                                            major for kind::f16): no transposed copy of P
+        dW,db  = [X * u, u]16^T . P16 * max|upstream|       both operands MN-major (TMA-loaded as stored,
+                                                            read transposed by wgmma): no transposed copy of P
     The upstream per-row gradient u = upstream / max|upstream| rides in the fp16 copy of X for dW and in
     the fp32 epilogue for dX, so P itself stays unnormalised."""
 
@@ -964,7 +964,7 @@ class _MHADrop(torch.autograd.Function):
 
 
 class _MHATensorCore(torch.autograd.Function):
-    """The attention core as batched tcgen05 products (csrc/mha_tc.cu): softmax and its backward in the GEMM
+    """The attention core as batched wgmma products (csrc/mha_tc.cu): softmax and its backward in the GEMM
     epilogues, all (sentence, head) pairs in one launch per product.  TF32 operands."""
 
     @staticmethod
@@ -1089,7 +1089,7 @@ def conv3x3_bias_relu(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torc
     x, w, b = _f32(x.detach()).contiguous(), _f32(w.detach()).contiguous(), _f32(b.detach())
     y = torch.empty(n, h, wd, cout, device=x.device, dtype=torch.float32)
     if _GEMM_BACKEND != lib.GEMM_SIMT and cout % 4 == 0:
-        # tensor-core path: patch matrix (im2col) x filter matrix [9*Cin, Cout] through the tcgen05
+        # tensor-core path: patch matrix (im2col) x filter matrix [9*Cin, Cout] through the wgmma
         # GEMM with the bias + ReLU epilogue; the output rows ARE the NHWC pixels.  The patch matrix
         # is built for a few images at a time so it stays below ~768 MB.
         k = 9 * cin

@@ -17,7 +17,7 @@ def device() -> torch.device:
     if _device is None:
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "neuralmonkey_b200 needs a CUDA device (sm_100a); no CPU fallback exists")
+                "neuralmonkey_b200 needs a CUDA device (sm_90a, H100); no CPU fallback exists")
         local_rank = int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(local_rank)
         _device = torch.device("cuda", local_rank)

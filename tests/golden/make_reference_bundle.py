@@ -30,6 +30,31 @@ LATE_FILES = ["tests/factored.ini", "tests/post-edit.ini", "tests/language-model
               "tests/data/val.tc.en"]
 
 
+# what the CPU replays of tests_run.sh need beyond the two bundles above (tests/test_reference_tests_run_cpu.py,
+# tests/test_reference_inis_cpu.py): small.ini, the run-time dataset INIs, the ten-sentence test corpus and the
+# captions / image lists of the flickr30k sample (its .npz feature maps are too large to bundle; the test writes
+# seeded stand-ins of the same shape)
+RUN_FILES = ["tests/data/flickr30k/train.de", "tests/data/flickr30k/val.de", "tests/data/flickr30k/train_images.npz.txt",
+             "tests/data/flickr30k/val_images.npz.txt",
+             "tests/small.ini", "tests/test_data.ini", "tests/beamsearch_ensembles.ini",
+             "tests/test_data_ensembles_single.ini", "tests/test_data_ensembles_duplicate.ini",
+             "tests/test_data_ensembles_all.ini", "tests/data/val10.tc.en", "tests/data/val10.tc.de",
+             "tests/data/val10.part1.tc.en", "tests/data/val10.part2.tc.en"]
+BUNDLES = ("reference_experiments.json", "reference_experiments_late.json", "reference_experiments_run.json")
+
+
+def unpack(tree: str) -> None:
+    """Every bundle into `tree` (tests/*.ini and tests/data/ as in the reference's tree)."""
+    for name in BUNDLES:
+        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), name), encoding="utf-8") as handle:
+            bundle = json.load(handle)
+        for rel, text in bundle["files"].items():
+            path = os.path.join(tree, rel)
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            with open(path, "w", encoding="utf-8") as handle:
+                handle.write(text)
+
+
 def write(files, name) -> None:
     bundle = {"source": "ufal/neuralmonkey @ 8b1465270f6bb28d5417a85cec492f7179036ede", "files": {}}
     for rel in files:
@@ -44,6 +69,7 @@ def write(files, name) -> None:
 def main() -> None:
     write(FILES, "reference_experiments.json")
     write(LATE_FILES, "reference_experiments_late.json")
+    write(RUN_FILES, "reference_experiments_run.json")
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""nm_gemm on the GPU: tcgen05/TMA path and CUDA-core path against an fp64 product."""
+"""nm_gemm on the GPU: wgmma/TMA path and CUDA-core path against an fp64 product."""
 import pytest
 import torch
 

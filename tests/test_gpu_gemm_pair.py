@@ -1,4 +1,4 @@
-"""CTA-pair tiles (tcgen05.mma.cta_group::2, 256 x BN per pair of SMs) of the tcgen05 products.
+"""CTA-pair tiles of the wgmma products (a cluster of two CTAs per 256 x BN tile, the B tile multicast to both).
 
 A pair computes exactly the products and sums of the one-CTA instance (same operands, same K order), so
 every family is run with `nm_gemm_set_pair_mode(0)` and `(1)` on the same inputs and compared bit for bit,

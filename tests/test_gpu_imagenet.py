@@ -45,7 +45,7 @@ def _params(model):
                                         ("vgg_16/conv5/conv5_3", 32)])
 @pytest.mark.parametrize("backend,rtol", [("simt", 2e-5), ("auto", 5e-3)])
 def test_vgg_stack_matches_oracle(layer, size, backend, rtol):
-    """simt: implicit-GEMM convolution on the CUDA cores (exact fp32); auto: im2col + tcgen05 GEMM
+    """simt: implicit-GEMM convolution on the CUDA cores (exact fp32); auto: im2col + wgmma GEMM
     with the bias+ReLU epilogue (TF32 operands)."""
     from neuralmonkey_b200 import ops
     ops.set_gemm_backend(backend)

@@ -1,4 +1,4 @@
-"""K8 on the tensor cores (csrc/mha_tc.cu): attention as batched tcgen05 products with the softmax and its
+"""K8 on the tensor cores (csrc/mha_tc.cu): attention as batched wgmma products with the softmax and its
 backward in the GEMM epilogues, against an fp64 restatement of attention/scaled_dot_product.py:160-214 (masking
 order, -1e9 replacement, dropout on the weights) and against the exact fp32 kernels.  TF32 operands: 10-bit
 mantissas, so the bar is relative 3e-3 / 5e-3 on outputs / gradients and 2e-3 absolute on the probabilities."""

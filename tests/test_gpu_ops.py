@@ -54,12 +54,12 @@ def test_layer_norm_fwd_bwd(dims):
                                   (3, 5, 8, 100)])
 @pytest.mark.parametrize("engine", ["exact", "tc"])
 def test_gru_layer_fwd_bwd(reverse, use_lengths, dims, engine):
-    """engine 'exact': fp32 CUDA-core recurrence; 'tc': tcgen05 recurrence (TF32 operands)."""
-    from neuralmonkey_b200 import lib, ops
-    ops.set_gemm_backend("simt")
+    """engine 'exact': every product in fp32 on the CUDA cores; 'tc': the default engine - the hoisted input
+    projections on the TF32 tensor-core GEMM wherever the shape is TMA-addressable, the recurrence on the cluster
+    kernels."""
+    from neuralmonkey_b200 import ops
+    ops.set_gemm_backend("simt" if engine == "exact" else "auto")
     tol, gtol = (2e-5, 5e-5) if engine == "exact" else (3e-3, 1e-2)
-    if engine == "tc":
-        lib.call("nm_gru_set_mode", 0)
     try:
         bsz, steps, e, h = dims
         g = torch.Generator().manual_seed(2)

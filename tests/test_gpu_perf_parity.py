@@ -1,4 +1,4 @@
-"""The BENCHED engine (default `auto` backend: tcgen05 fp16 / TF32 products, tensor-core GRU recurrence)
+"""The BENCHED engine (default `auto` backend: wgmma fp16 / TF32 products, cluster GRU recurrence)
 against the fp32 oracle at the PERF dimensions of BASELINE.json - the bar north_star states: train loss within
 1e-3.  Parameters are random at a scale that makes every activation matter (the initialisers would leave the
 logits at ~0 and the loss at log V whatever the arithmetic does)."""

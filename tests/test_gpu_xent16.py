@@ -72,7 +72,7 @@ def test_gemm_f16(m, n, k, transposed, beta):
 @pytest.mark.parametrize("m,n,k", [(64, 64, 64), (301, 1000, 1100), (301, 4100, 12800), (130, 96, 72), (40, 260, 8200)])
 @pytest.mark.parametrize("beta", [0.0, 1.0])
 def test_gemm_f16_tn(m, n, k, beta):
-    """C[M,N] = alpha * A^T . B with A [K,M], B [K,N] stored reduction-major (MN-major tcgen05 operands)."""
+    """C[M,N] = alpha * A^T . B with A [K,M], B [K,N] stored reduction-major (MN-major operands)."""
     lib = _lib()
     g = torch.Generator().manual_seed(3)
     mp, np_ = (m + 7) // 8 * 8, (n + 7) // 8 * 8

@@ -6,7 +6,7 @@ Written after round 2's GPU budget was spent: the host composition is checked on
 operations (tests/test_host_model_cpu.py::test_rnn_decoder_with_scaled_dot_attention_objects) and every
 operation it calls is GPU-verified in other compositions (the Transformer decoder's cross-attention makes the same
 `ops.mha_core` call), but THIS test has never run.  It is therefore opt-in - `NMB200_RUN_UNRUN_GPU_TESTS=1` -
-so that the suite the driver runs holds only tests that have been seen green on a B200; `bench.py` runs it in a
+so that the default suite holds only tests that have been seen green on a GPU; `bench.py` runs it in a
 separate process and records the outcome under `extra_workloads.late_gpu_checks`."""
 import os
 

@@ -1,4 +1,5 @@
 """Host-side logic that needs no GPU: vocabulary, padding, arena layout, sharding."""
+import json
 import os
 import subprocess
 import sys
@@ -263,6 +264,8 @@ for name in cpu_ops.STAND_INS:
     setattr(ops, name, getattr(cpu_ops, name))
 runtime._device = torch.device("cpu")
 GenericTrainer._adam_kernel = cpu_ops.adam_kernel
+from neuralmonkey_b200 import distributed
+distributed.init_from_env(backend="gloo")     # CPU tensors: gloo even where a GPU (and with it NCCL) is present
 sys.argv = ["neuralmonkey-train", {ini!r}]
 from neuralmonkey_b200.train import main
 main()
@@ -458,8 +461,8 @@ def test_model_part_save_and_load(tmp_path, monkeypatch):
 def test_word2vec_files_and_the_perplexity_evaluator(tmp_path):
     """util/word2vec.py (vocabulary + embedding initialiser from a word2vec text file: special tokens first,
     zeros unless the file has them) and evaluators.PerplexityEvaluator (2 ** mean of the non-zero
-    cross-entropies), as tests/language-model.ini uses them; compared with the reference's module when the
-    reference tree is there."""
+    cross-entropies), as tests/language-model.ini uses them; compared with what the reference's module loads
+    from its sample file."""
     import numpy as np
     from neuralmonkey_b200.evaluators import PerplexityEvaluator
     from neuralmonkey_b200.util import word2vec
@@ -481,17 +484,15 @@ def test_word2vec_files_and_the_perplexity_evaluator(tmp_path):
     ppl = PerplexityEvaluator("perplexity")
     assert ppl([[1.0, 3.0, 0.0], [2.0, 0.0, 0.0]], [[], []]) == 2 ** 2.0
     assert ppl([[0.0]], [[]]) != ppl([[0.0]], [[]])          # NaN: nothing counted
-    sample = "/root/reference/tests/data/sample.w2v"
-    module = "/root/reference/neuralmonkey/util/word2vec.py"
-    if os.path.exists(sample) and os.path.exists(module):
-        code = open(module).read().replace("from typeguard import check_argument_types", "") \
-            .replace("from neuralmonkey.vocabulary import", "from neuralmonkey_b200.vocabulary import") \
-            .replace("check_argument_types()", "").replace("np.float)", "np.float64)")
-        ref = {}
-        exec(compile(code, module, "exec"), ref)            # the reference's own loader, its imports redirected
-        theirs, ours = ref["Word2Vec"](sample), word2vec.Word2Vec(sample)
-        assert np.array_equal(theirs.embeddings, ours.embeddings)
-        assert theirs.vocabulary.index_to_word == ours.vocabulary.index_to_word
+    # the reference's own loader on its sample file (tests/golden/make_word2vec_golden.py)
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+    with open(os.path.join(golden, "reference_experiments_late.json"), encoding="utf-8") as handle:
+        (tmp_path / "sample.w2v").write_text(json.load(handle)["files"]["tests/data/sample.w2v"])
+    with open(os.path.join(golden, "word2vec_golden.json"), encoding="utf-8") as handle:
+        theirs = json.load(handle)
+    ours = word2vec.Word2Vec(str(tmp_path / "sample.w2v"))
+    assert np.array_equal(np.array(theirs["embeddings"], dtype=ours.embeddings.dtype), ours.embeddings)
+    assert theirs["index_to_word"] == ours.vocabulary.index_to_word
 
 
 def test_model_part_reuse_shares_variables():

@@ -1,25 +1,23 @@
 """The reference's OWN experiment INIs for the hot path (tests/{bahdanau,transformer,beamsearch,small,
-factored,post-edit}.ini of /root/reference, the ones `tests/tests_run.sh` trains), unchanged, through this package's
+factored,post-edit,language-model}.ini of the reference, the ones its `tests/tests_run.sh` trains), unchanged, through this package's
 `neuralmonkey-train` entry point - on the CPU over the stand-in operations of tests/cpu_ops.py.
 What is exercised is everything but the kernels: the INI grammar with variables and environment
 substitution, `class=` resolution against this package, constructor signatures and validation, datasets
 with bucketing, vocabularies, the training loop with validation, runners, evaluators, checkpoints.
-Only the output locations are redirected (the reference tree is read-only), and `evaluators.TER`
-(third-party pyter, absent here as TensorFlow is) is dropped from small.ini's evaluation list.
-
-Skipped when /root/reference is not there (it exists in the build container only)."""
+The INIs and their toy corpora come from the bundles under tests/golden/ (make_reference_bundle.py), unpacked
+into a scratch tree.  Only the output locations are redirected, and `evaluators.TER` (third-party pyter, absent
+here as TensorFlow is) is dropped from small.ini's evaluation list."""
 import os
 import sys
 
+import numpy as np
 import pytest
 import torch
 
 from tests import cpu_ops
+from tests.golden.make_reference_bundle import unpack
 
-REFERENCE = "/root/reference"
-pytestmark = [pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, "tests", "data")),
-                                 reason="the reference tree is not mounted"),
-              pytest.mark.filterwarnings("ignore:Converting a tensor with requires_grad")]
+pytestmark = [pytest.mark.filterwarnings("ignore:Converting a tensor with requires_grad")]
 
 CASES = {
     "bahdanau": ['val_data_no_target.outputs=[("encoded", "{out}/encoded"), ("debugtensors", "{out}/debugtensors")]'],
@@ -47,7 +45,8 @@ def test_reference_ini_trains_unchanged(monkeypatch, tmp_path, name):
     monkeypatch.setenv("NMB200_UNVERIFIED", "1")          # small.ini: Nematus GRU cells, conditional GRU
     monkeypatch.setenv("NEURALMONKEY_STRICT", "1")        # as tests_run.sh: warnings are errors
     monkeypatch.setenv("NM_EXPERIMENT_NAME", "small")     # small.ini reads it from the environment
-    monkeypatch.chdir(REFERENCE)                          # the INIs name their data relative to the tree
+    unpack(str(tmp_path / "tree"))
+    monkeypatch.chdir(tmp_path / "tree")                  # the INIs name their data relative to the tree
     out = str(tmp_path / name)
     argv = ["neuralmonkey-train", "tests/{}.ini".format(name), "-s", 'main.output="{}"'.format(out)]
     for change in CASES[name]:
@@ -152,8 +151,9 @@ output_series="target"
 
 def test_captioning_over_the_reference_feature_files(monkeypatch, tmp_path):
     """The image half of the reference's tests/flat-multiattention.ini - `readers.numpy_reader.from_file_list`
-    over its flickr30k .npz feature maps into a `SpatialFiller` - under the attention decoder of the hot path
-    (the FlatMultiAttention wrapper of that INI is outside it)."""
+    over the flickr30k sample's file lists into a `SpatialFiller` - under the attention decoder of the hot path
+    (the FlatMultiAttention wrapper of that INI is outside it).  The 8 x 8 x 2048 feature maps are seeded
+    stand-ins written in the layout of the reference's .npz files (one `arr_0` array each)."""
     from neuralmonkey_b200 import ops, runtime
     from neuralmonkey_b200.trainers.generic_trainer import GenericTrainer
     for op in cpu_ops.STAND_INS:
@@ -161,7 +161,14 @@ def test_captioning_over_the_reference_feature_files(monkeypatch, tmp_path):
     monkeypatch.setattr(runtime, "_device", torch.device("cpu"))
     monkeypatch.setattr(GenericTrainer, "_adam_kernel", cpu_ops.adam_kernel)
     monkeypatch.setenv("NEURALMONKEY_STRICT", "1")
-    monkeypatch.chdir(REFERENCE)
+    tree = tmp_path / "tree"
+    unpack(str(tree))
+    flickr = tree / "tests" / "data" / "flickr30k"
+    g = np.random.default_rng(30)
+    for listing in ("train_images.npz.txt", "val_images.npz.txt"):
+        for name in (flickr / listing).read_text().split():
+            np.savez(str(flickr / name), g.standard_normal((8, 8, 2048)).astype(np.float32))
+    monkeypatch.chdir(tree)
     out = str(tmp_path / "features")
     ini = tmp_path / "features.ini"
     ini.write_text(_FEATURES_INI.format(out=out))

@@ -1,6 +1,6 @@
 """The in-scope part of the reference's own integration script, tests/tests_run.sh, command by command and with
-the INIs TRULY unchanged - output directories included: the commands run from a scratch directory whose
-`tests/*.ini` and `tests/data` are symbolic links into /root/reference and whose `tests/outputs` is real, so
+the INIs TRULY unchanged - output directories included: the commands run from a scratch directory into which
+the reference's `tests/*.ini` and `tests/data` files are unpacked from the bundles under tests/golden/, so
 `neuralmonkey-run` finds what `neuralmonkey-train` wrote where the INI says.  On the CPU over the stand-in
 operations (tests/cpu_ops.py); what is exercised is the whole host side of both entry points.
 
@@ -15,7 +15,7 @@ operations (tests/cpu_ops.py); what is exercised is the whole host side of both 
     bin/neuralmonkey-run tests/beamsearch_ensembles.ini tests/test_data_ensembles_all.ini
 
 (The other training commands of the script that are on the hot path - bahdanau, post-edit, factored,
-language-model - are in tests/test_reference_inis_cpu.py.)  Skipped when /root/reference is not there."""
+language-model - are in tests/test_reference_inis_cpu.py.)"""
 import importlib
 import json
 import os
@@ -25,11 +25,9 @@ import pytest
 import torch
 
 from tests import cpu_ops
+from tests.golden.make_reference_bundle import unpack
 
-REFERENCE = "/root/reference"
-pytestmark = [pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, "tests", "data")),
-                                 reason="the reference tree is not mounted"),
-              pytest.mark.filterwarnings("ignore:Converting a tensor with requires_grad")]
+pytestmark = [pytest.mark.filterwarnings("ignore:Converting a tensor with requires_grad")]
 
 
 @pytest.fixture
@@ -43,10 +41,7 @@ def scratch_tree(monkeypatch, tmp_path):
     monkeypatch.setenv("NEURALMONKEY_STRICT", "1")
     tests_dir = tmp_path / "tests"
     (tests_dir / "outputs").mkdir(parents=True)
-    os.symlink(os.path.join(REFERENCE, "tests", "data"), str(tests_dir / "data"))
-    for name in os.listdir(os.path.join(REFERENCE, "tests")):
-        if name.endswith(".ini"):
-            os.symlink(os.path.join(REFERENCE, "tests", name), str(tests_dir / name))
+    unpack(str(tmp_path))
     monkeypatch.chdir(tmp_path)
 
     def command(kind, *argv):

@@ -1,7 +1,7 @@
 """Per-shape GPU time of nm_gemm for the products of the en-de and Transformer training steps.
 
 Every shape is launched back to back REPS times between two CUDA events, operands rotating through enough
-buffer sets to exceed the 126 MB L2 (so A and C come from / go to HBM as they do inside a step, while the
+buffer sets to exceed the 50 MB L2 (so A and C come from / go to HBM as they do inside a step, while the
 small weight operand stays L2-resident as it does inside a step).  Prints one line per shape:
 time per launch, TFLOP/s, and the HBM floor (bytes of A, B and C once each at the measured copy rate).
 
@@ -37,9 +37,9 @@ TRANSFORMER = [
 # what a launch costs by itself, one tile per SM with a short and with a long reduction (steady-state rate of the
 # TMA ring per SM), and the same through a pure-L2 operand set
 DIAG = [
-    ("1 tile      ", 0, 1, 128, 128, 32), ("148 tiles k=1 blk", 0, 1, 18944, 128, 32),
-    ("148 tiles K=320 ", 0, 1, 18944, 128, 320), ("148 tiles K=3200", 0, 1, 18944, 128, 3200),
-    ("148 tiles K=320 BN256", 0, 1, 18944, 256, 320), ("148 tiles K=3200 BN256", 0, 1, 18944, 256, 3200),
+    ("1 tile      ", 0, 1, 128, 128, 32), ("132 tiles k=1 blk", 0, 1, 16896, 128, 32),
+    ("132 tiles K=320 ", 0, 1, 16896, 128, 320), ("132 tiles K=3200", 0, 1, 16896, 128, 3200),
+    ("132 tiles K=320 BN256", 0, 1, 16896, 256, 320), ("132 tiles K=3200 BN256", 0, 1, 16896, 256, 3200),
     ("4 rounds K=320", 0, 1, 75776, 128, 320), ("4 rounds K=320 MN-B", 0, 0, 75776, 128, 320),
 ]
 

@@ -23,7 +23,7 @@ def run(B, budget, reps=3):
 print("resident clusters fwd/bwd:", lib.load().nm_gru_resident_clusters(0), lib.load().nm_gru_resident_clusters(1))
 prof = torch.zeros(8, dtype=torch.int64, device="cuda")
 lib.load().nm_gru_debug_profile(prof.data_ptr())
-for B, budget in ((16, 8), (256, 148)):
+for B, budget in ((16, 8), (256, 132)):
     ms = run(B, budget)
     print("B=%4d budget=%3d -> %.3f ms  (%.1f us/step)" % (B, budget, ms, ms * 1000 / T), flush=True)
     c = prof.cpu().tolist(); prof.zero_()

@@ -3,7 +3,7 @@ BASELINE.json: text files on disk, an INI, the package's own training loop (data
 index, pinned upload, the captured training step).  What bench.py's `e2e` measures starts at id tensors in pinned
 host memory; this starts at words.
 
-    python tools/ini_loop_bench.py                       # B200: 30 steps of 256 sentences x 50 tokens, V = 32000
+    python tools/ini_loop_bench.py                       # 30 steps of 256 sentences x 50 tokens, V = 32000
     python tools/ini_loop_bench.py --standins --rnn 16 --vocab 300 --sentences 96 --batch 16    # host logic, CPU
 
 The corpus is synthetic (uniform random words, fixed length, as in bench.py); logging and validation periods are
