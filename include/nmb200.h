@@ -86,6 +86,14 @@ int nm_gemm_set_pair_mode(int mode);
 int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K,
                     int64_t lda, int64_t ldb, int64_t ldc);
 
+/* dst[c * ld_dst + r] = tf32(src[r * ld_src + c]) for a [rows, cols] source (a strided column slice is fine):
+ * the transpose of src rounded to TF32 with cvt.rna (low 13 bits zero), i.e. the K-major copy of an operand
+ * whose reduction dimension is strided, which the wgmma GEMM then loads by TMA with the same operand bits its
+ * producer threads would have made.  ld_dst >= rows and a multiple of 4 (TMA-addressable rows); the padding
+ * columns [rows, ld_dst) of dst are not written.  HBM-bound: 64 x 64 tiles through shared memory, 16-byte
+ * loads / stores where pitches and bases allow. */
+int nm_transpose_tf32(const float* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t rows,
+                      int64_t cols, void* stream);
 /* dx = dy * act'(y) expressed through the activation OUTPUT y (tanh: 1-y^2,
  * relu: y>0, sigmoid: y(1-y)); n elements; dx may alias dy. */
 int nm_act_bwd(const float* y, const float* dy, float* dx, int64_t n, int act,

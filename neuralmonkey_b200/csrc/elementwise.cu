@@ -109,6 +109,65 @@ __global__ void maxout_bwd_kernel(const float* __restrict__ dy, const uint8_t* _
 }
 
 // ---------------------------------------------------------------------------
+// K-major TF32 copies for the tensor-core GEMM: wgmma reads TF32 operands K-major only, and a K-major operand
+// arrives by TMA.  dst[c, r] = tf32_rna(src[r, c]) through a 64 x 64 tile in shared memory: each source row
+// segment is read with 16-byte loads (16 threads per row), each destination row segment written with 16-byte
+// stores (16 threads per row); scalar accesses where a pitch, a base or the edge of the matrix does not allow a
+// vector.  The rounding is the producer threads' cvt.rna.tf32 (low 13 bits cleared), so the GEMM sees the same
+// operand bits either way.
+// ---------------------------------------------------------------------------
+constexpr int TT_EDGE = 64;
+
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t u;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+  return __uint_as_float(u & 0xffffe000u);
+}
+
+__global__ void __launch_bounds__(256) transpose_tf32_kernel(const float* __restrict__ src, int64_t ld_src,
+                                                             float* __restrict__ dst, int64_t ld_dst, int64_t rows,
+                                                             int64_t cols, bool vec_in, bool vec_out) {
+  __shared__ float tile[TT_EDGE][TT_EDGE + 1];     // [source column][source row]: 2-way bank conflicts at most
+  const int64_t r0 = (int64_t)blockIdx.x * TT_EDGE, c0 = (int64_t)blockIdx.y * TT_EDGE;
+  const int q = threadIdx.x & 15, sub = threadIdx.x >> 4;
+#pragma unroll
+  for (int i = 0; i < TT_EDGE; i += 16) {
+    const int lr = sub + i;
+    const int64_t r = r0 + lr, c = c0 + 4 * q;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (r < rows) {
+      const float* p = src + r * ld_src + c;
+      if (vec_in && c + 4 <= cols) {
+        const float4 x = __ldg(reinterpret_cast<const float4*>(p));
+        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (c + j < cols) v[j] = __ldg(p + j);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tile[4 * q + j][lr] = tf32_rna(v[j]);
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < TT_EDGE; i += 16) {
+    const int lc = sub + i;
+    const int64_t c = c0 + lc, r = r0 + 4 * q;
+    if (c >= cols || r >= rows) continue;
+    float* p = dst + c * ld_dst + r;
+    const float* t = tile[lc] + 4 * q;
+    if (vec_out && r + 4 <= rows) {
+      *reinterpret_cast<float4*>(p) = make_float4(t[0], t[1], t[2], t[3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (r + j < rows) p[j] = t[j];
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
 // K7 layer norm: one warp per row, the row cached in registers (PER_LANE values per
 // lane, D <= 32*PER_LANE).  Parameter gradients are a separate column reduction.
 // ---------------------------------------------------------------------------
@@ -395,6 +454,24 @@ int nm_maxout_bwd(const float* dy, const uint8_t* which, float* dz, int64_t M, i
   if (M == 0) return NM_OK;
   maxout_bwd_kernel<<<grid_for(M * O, 256), 256, 0, (cudaStream_t)stream>>>(dy, which, dz, M, O);
   NM_LAUNCH_CHECK("nm_maxout_bwd");
+  return NM_OK;
+}
+
+int nm_transpose_tf32(const float* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t rows, int64_t cols,
+                      void* stream) {
+  NM_REQUIRE(src && dst, NM_E_INVALID, "nm_transpose_tf32: null pointer");
+  NM_REQUIRE(rows >= 0 && cols >= 0 && ld_src >= cols && ld_dst >= rows && ld_dst % 4 == 0, NM_E_INVALID,
+             "nm_transpose_tf32: bad sizes (rows=%lld cols=%lld ld_src=%lld ld_dst=%lld)", (long long)rows,
+             (long long)cols, (long long)ld_src, (long long)ld_dst);
+  if (rows == 0 || cols == 0) return NM_OK;
+  const int64_t gx = ceil_div(rows, TT_EDGE), gy = ceil_div(cols, TT_EDGE);
+  NM_REQUIRE(gx <= 0x7fffffffLL && gy <= 65535, NM_E_UNSUPPORTED, "nm_transpose_tf32: %lld x %lld is too large",
+             (long long)rows, (long long)cols);
+  const bool vec_in = ld_src % 4 == 0 && (uintptr_t)src % 16 == 0;
+  const bool vec_out = (uintptr_t)dst % 16 == 0;
+  transpose_tf32_kernel<<<dim3((unsigned)gx, (unsigned)gy), 256, 0, (cudaStream_t)stream>>>(
+      src, ld_src, dst, ld_dst, rows, cols, vec_in, vec_out);
+  NM_LAUNCH_CHECK("nm_transpose_tf32");
   return NM_OK;
 }
 

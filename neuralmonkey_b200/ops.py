@@ -49,10 +49,43 @@ def _rows(t: torch.Tensor) -> Tuple[torch.Tensor, int]:
     return t, ld
 
 
+def kmajor_tf32(t: torch.Tensor) -> torch.Tensor:
+    """t^T rounded to TF32 (cvt.rna): a [cols, rows] view of a fresh buffer whose row pitch is a multiple of 4 floats
+    (nm_transpose_tf32).  The K-major form of a GEMM operand whose reduction dimension is strided."""
+    t, ld = _rows(_f32(t))
+    rows, cols = t.shape
+    ld_t = (rows + 3) // 4 * 4
+    buf = torch.empty(cols, ld_t, device=t.device, dtype=torch.float32)
+    call("nm_transpose_tf32", ptr(t), ld, ptr(buf), ld_t, rows, cols, lib.stream())
+    return buf[:, :rows]
+
+
+def _on_tensor_cores(trans_a: bool, trans_b: bool, m: int, n: int, k: int, a: torch.Tensor, lda: int,
+                     b: torch.Tensor, ldb: int, backend: int) -> bool:
+    """nm_gemm's own choice of engine: wgmma unless the backend is the exact one or the operands are not
+    TMA-addressable (row pitches multiples of 4 floats, 16-byte aligned bases)."""
+    return (backend != lib.GEMM_SIMT and m > 0 and n > 0 and k > 0
+            and lib.load().nm_gemm_uses_tc(int(trans_a), int(trans_b), m, n, k, lda, ldb, n) == 1
+            and a.data_ptr() % 16 == 0 and b.data_ptr() % 16 == 0)
+
+
+def _tn_on_tensor_cores(x: torch.Tensor, dy: torch.Tensor) -> bool:
+    """Whether the weight-gradient product x^T . dy (both stored [K, *]) runs on the tensor cores."""
+    x, ldx = _rows(x)
+    dy, ldy = _rows(dy)
+    return _on_tensor_cores(True, False, x.size(1), dy.size(1), x.size(0), x, ldx, dy, ldy, _GEMM_BACKEND)
+
+
 def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, trans_a: bool = False,
          trans_b: bool = False, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
          beta: float = 0.0, backend: Optional[int] = None) -> torch.Tensor:
-    """out = act(op(a) @ op(b) + bias) + beta*out, all through nm_gemm (no torch math)."""
+    """out = act(op(a) @ op(b) + bias) + beta*out, all through nm_gemm (no torch math).
+
+    On the tensor-core path an operand stored MN-major (a with trans_a, b without trans_b) is handed over as its
+    K-major TF32 copy (kmajor_tf32), which the kernel loads by TMA: wgmma reads TF32 operands K-major only, and the
+    kernel's own way of reading MN-major ones - its producer threads transposing every tile - is several times
+    slower.  The copy carries the operand bits those threads would make, so the result is the same.  The exact
+    engine always reads the operands as given."""
     a, lda = _rows(_f32(a))
     b, ldb = _rows(_f32(b))
     if out.dim() != 2 or (out.stride(1) != 1 and out.size(1) != 1):
@@ -63,9 +96,16 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, trans_a: bool = Fa
     if k != kb or out.size(0) != m or out.size(1) != n:
         raise ValueError("gemm shape mismatch: op(a) [{},{}] op(b) [{},{}] out {}".format(
             m, k, kb, n, tuple(out.shape)))
+    backend = _GEMM_BACKEND if backend is None else backend
+    if (trans_a or not trans_b) and _on_tensor_cores(trans_a, trans_b, m, n, k, a, lda, b, ldb, backend):
+        if trans_a:
+            a, lda = _rows(kmajor_tf32(a))
+            trans_a = False
+        if not trans_b:
+            b, ldb = _rows(kmajor_tf32(b))
+            trans_b = True
     call("nm_gemm", int(trans_a), int(trans_b), m, n, k, ptr(a), lda, ptr(b), ldb, ptr(out), ldc,
-         ptr(bias), lib.NM_ACT[act], float(beta),
-         _GEMM_BACKEND if backend is None else backend, lib.stream())
+         ptr(bias), lib.NM_ACT[act], float(beta), backend, lib.stream())
     return out
 
 
@@ -116,29 +156,50 @@ def _off_the_chain(fn, *operands) -> None:
     _wg["keep"].append(operands)
 
 
-def _gru_weight_grads(x2, hp2, rh2, dzg, dzc, wg, wc, e, sinks):
-    """Weight / bias gradients of one GRU direction (rows [:E] of the kernels from x, rows [E:] from the recurrent
-    operand).  With all four variables in the gradient buffer the six launches leave the backward chain
-    (`_off_the_chain`) and nothing is returned; otherwise (dWg, dbg, dWc, dbc) with None for buffered ones."""
-    sg, sbg, sc, sbc = sinks
+def _gru_weight_grads(x2, directions, e, h):
+    """Weight / bias gradients of the directions of a GRU layer over one input x2 [B*T, E].  A direction is
+    (hprev [B*T, H], rh [B*T, H], dxproj [B*T, 3H], wg, wc, sinks); rows [:E] of its kernels come from x2, rows
+    [E:] from the recurrent operand, against dzg = dxproj[:, :2H] and dzc = dxproj[:, 2H:].  With every variable
+    in the gradient buffer all launches leave the backward chain (`_off_the_chain`) and a None 4-tuple per
+    direction is returned; otherwise (dWg, dbg, dWc, dbc) per direction with None for buffered ones.
 
-    def products(dwg, dwc, beta_g, beta_c):
-        gemm(x2, dzg, dwg[:e], trans_a=True, beta=beta_g)
-        gemm(hp2, dzg, dwg[e:], trans_a=True, beta=beta_g)
-        gemm(x2, dzc, dwc[:e], trans_a=True, beta=beta_c)
-        gemm(rh2, dzc, dwc[e:], trans_a=True, beta=beta_c)
-    if sg is not None and sbg is not None and sc is not None and sbc is not None:
+    On the tensor cores the products take K-major TF32 copies (see `gemm`), each made once: x2 for all the
+    directions, dxproj per direction (dzg^T and dzc^T are row ranges of its copy), hprev and rh."""
+    def products(outs):
+        x2t = None
+        for (hp2, rh2, dxp, _wg, _wc, _sinks), (dwg, dwc, beta_g, beta_c) in zip(directions, outs):
+            dzg, dzc = dxp[:, :2 * h], dxp[:, 2 * h:]
+            if all(_tn_on_tensor_cores(x, dz) for x, dz in ((x2, dzg), (hp2, dzg), (x2, dzc), (rh2, dzc))):
+                if x2t is None:
+                    x2t = kmajor_tf32(x2)
+                dxpt = kmajor_tf32(dxp)
+                x, hp, rh, dg, dc = x2t, kmajor_tf32(hp2), kmajor_tf32(rh2), dxpt[:2 * h], dxpt[2 * h:]
+                trans = (False, True)       # x^T . dz = (x^T) . (dz^T)^T
+            else:
+                x, hp, rh, dg, dc = x2, hp2, rh2, dzg, dzc
+                trans = (True, False)
+            gemm(x, dg, dwg[:e], *trans, beta=beta_g)
+            gemm(hp, dg, dwg[e:], *trans, beta=beta_g)
+            gemm(x, dc, dwc[:e], *trans, beta=beta_c)
+            gemm(rh, dc, dwc[e:], *trans, beta=beta_c)
+
+    if all(s is not None for d in directions for s in d[5]):
         def into_the_buffer():
-            products(sg, sc, 1.0, 1.0)
-            _bias_grad(dzg, sbg)
-            _bias_grad(dzc, sbc)
-        _off_the_chain(into_the_buffer, x2, hp2, rh2, dzg, dzc)
-        return None, None, None, None
-    dwg = sg if sg is not None else torch.empty_like(wg)
-    dwc = sc if sc is not None else torch.empty_like(wc)
-    products(dwg, dwc, 1.0 if sg is not None else 0.0, 1.0 if sc is not None else 0.0)
-    return (None if sg is not None else dwg, _bias_grad(dzg, sbg), None if sc is not None else dwc,
-            _bias_grad(dzc, sbc))
+            products([(sg, sc, 1.0, 1.0) for sg, _, sc, _ in (d[5] for d in directions)])
+            for d in directions:
+                _bias_grad(d[2][:, :2 * h], d[5][1])
+                _bias_grad(d[2][:, 2 * h:], d[5][3])
+        _off_the_chain(into_the_buffer, x2, *(t for d in directions for t in d[:3]))
+        return [(None, None, None, None)] * len(directions)
+    outs, grads = [], []
+    for hp2, rh2, dxp, wg, wc, (sg, sbg, sc, sbc) in directions:
+        dwg = sg if sg is not None else torch.empty_like(wg)
+        dwc = sc if sc is not None else torch.empty_like(wc)
+        outs.append((dwg, dwc, 1.0 if sg is not None else 0.0, 1.0 if sc is not None else 0.0))
+        grads.append((None if sg is not None else dwg, _bias_grad(dxp[:, :2 * h], sbg),
+                      None if sc is not None else dwc, _bias_grad(dxp[:, 2 * h:], sbc)))
+    products(outs)
+    return grads
 
 
 def _weight_grad(a: torch.Tensor, b: torch.Tensor, trans_a: bool, trans_b: bool,
@@ -235,7 +296,9 @@ class _Linear(torch.autograd.Function):
         w_sink, b_sink = ctx.sinks
         want_w, want_b = ctx.needs_input_grad[1], ctx.has_bias and ctx.needs_input_grad[2]
         if (want_w and w_sink is not None) and (not want_b or b_sink is not None):
-            def into_the_buffer():      # both accumulate into the gradient buffer: nothing to return
+            # both accumulate into the gradient buffer: nothing to return.  gemm makes the K-major copies of x2 and
+            # dpre here, so that they too run on the weight-gradient stream
+            def into_the_buffer():
                 _weight_grad(x2, dpre, True, False, w_sink, w.shape)
                 if want_b:
                     _bias_grad(dpre, b_sink)
@@ -484,8 +547,8 @@ class _GRULayer(torch.autograd.Function):
              ptr(gates), ptr(hprev), ptr(dstates), ptr(draw), ptr(dfinal), ptr(dxproj), ptr(dh0),
              ptr(work), bsz, t, h, int(ctx.sm_budget), lib.stream())
         dzg, dzc = dxproj[:, :2 * h], dxproj[:, 2 * h:]
-        dwg, dbg, dwc, dbc = _gru_weight_grads(x2, hprev.view(bsz * t, h), rh.view(bsz * t, h), dzg, dzc, wg, wc, e,
-                                               ctx.sinks)
+        [(dwg, dbg, dwc, dbc)] = _gru_weight_grads(
+            x2, [(hprev.view(bsz * t, h), rh.view(bsz * t, h), dxproj, wg, wc, ctx.sinks)], e, h)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(bsz * t, e, device=dev, dtype=torch.float32)
@@ -561,18 +624,15 @@ class _BiGRULayer(torch.autograd.Function):
              ptr(wg_f[e:]), ptr(wc_f[e:]), 0, ptr(ga_f), ptr(hp_f), ptr(dst_f), ptr(dfi_f), ptr(dxp_f),
              ptr(wg_b[e:]), ptr(wc_b[e:]), 1, ptr(ga_b), ptr(hp_b), ptr(dst_b), ptr(dfi_b), ptr(dxp_b),
              ptr(lengths), ptr(work), bsz, t, h, lib.stream())
-        grads = []
         dx = torch.empty(bsz * t, e, device=dev, dtype=torch.float32) if ctx.needs_input_grad[0] else None
-        first = True
-        for (wg, wc, hp, rh, dxp, sinks) in ((wg_f, wc_f, hp_f, rh_f, dxp_f, ctx.sinks[:4]),
-                                             (wg_b, wc_b, hp_b, rh_b, dxp_b, ctx.sinks[4:])):
-            dzg, dzc = dxp[:, :2 * h], dxp[:, 2 * h:]
-            if dx is not None:      # the chain first: the input gradient is what the older layers wait for
-                gemm(dzg, wg[:e], dx, trans_b=True, beta=0.0 if first else 1.0)
-                gemm(dzc, wc[:e], dx, trans_b=True, beta=1.0)
-                first = False
-            grads += list(_gru_weight_grads(x2, hp.view(bsz * t, h), rh.view(bsz * t, h), dzg, dzc, wg, wc, e, sinks))
-        return (dx.view(bsz, t, e) if dx is not None else None, None) + tuple(grads)
+        directions = ((wg_f, wc_f, hp_f, rh_f, dxp_f, ctx.sinks[:4]), (wg_b, wc_b, hp_b, rh_b, dxp_b, ctx.sinks[4:]))
+        if dx is not None:          # the chain first: the input gradient is what the older layers wait for
+            for i, (wg, wc, _hp, _rh, dxp, _sinks) in enumerate(directions):
+                gemm(dxp[:, :2 * h], wg[:e], dx, trans_b=True, beta=0.0 if i == 0 else 1.0)
+                gemm(dxp[:, 2 * h:], wc[:e], dx, trans_b=True, beta=1.0)
+        grads = _gru_weight_grads(x2, [(hp.view(bsz * t, h), rh.view(bsz * t, h), dxp, wg, wc, sinks)
+                                       for wg, wc, hp, rh, dxp, sinks in directions], e, h)
+        return (dx.view(bsz, t, e) if dx is not None else None, None) + tuple(g for d in grads for g in d)
 
 
 def gru_bilayer(x: torch.Tensor, lengths: torch.Tensor, cell_fw, cell_bw):
