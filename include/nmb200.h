@@ -77,11 +77,6 @@ int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K,
             const float* A, int64_t lda, const float* B, int64_t ldb,
             float* C, int64_t ldc, const float* bias, int act, float beta,
             int backend, void* stream);
-/* Tile shape of the wgmma products (nm_gemm, nm_gemm_f16, nm_logits_xent_*): 1 = a cluster of two CTAs per 256-row
- * tile wherever the shape allows (B K-major, 128 or 256 columns per tile): each CTA loads half of every B k-block
- * with a multicast TMA into both; 0 = one CTA per 128-row tile; -1 = the library's choice (default: one CTA;
- * NMB200_TC_PAIR presets it). */
-int nm_gemm_set_pair_mode(int mode);
 /* 1 if nm_gemm(AUTO) would take the wgmma path for this problem. */
 int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K,
                     int64_t lda, int64_t ldb, int64_t ldc);

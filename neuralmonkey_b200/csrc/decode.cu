@@ -178,7 +178,7 @@ int nm_decode_logits_step(const float* X, int64_t ldx, const float* W, int64_t l
   const DecodeSelect sel{finished_in, symbols_out, finished_out, mask_out, unfinished_count,
                          targets, weights, xent};
   const bool tc_ok = part && (reinterpret_cast<uintptr_t>(part) & 15) == 0 &&
-                     tc_gemm_supported(0, transW, M, V, K, ldx, ldw, V, X, W, nullptr);
+                     tc_gemm_supported(M, V, K, ldx, ldw, X, W);
   if (backend == NM_GEMM_TC)
     NM_REQUIRE(tc_ok, NM_E_UNSUPPORTED, "nm_decode_logits_step: operands not TMA-addressable or no scratch");
   if (tc_ok && backend != NM_GEMM_SIMT) {

@@ -27,13 +27,7 @@ extern "C" {
 
 int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K, int64_t lda,
                     int64_t ldb, int64_t ldc) {
-  return tc_gemm_supported(transA, transB, M, N, K, lda, ldb, ldc, nullptr, nullptr, nullptr) ? 1 : 0;
-}
-
-int nm_gemm_set_pair_mode(int mode) {
-  NM_REQUIRE(mode >= -1 && mode <= 1, NM_E_INVALID, "nm_gemm_set_pair_mode: mode must be -1 (policy), 0 or 1");
-  tc_gemm_set_pair_mode(mode);
-  return NM_OK;
+  return tc_gemm_supported(M, N, K, lda, ldb, nullptr, nullptr) ? 1 : 0;
 }
 
 int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
@@ -49,7 +43,7 @@ int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K, const float
   NM_REQUIRE(backend >= NM_GEMM_AUTO && backend <= NM_GEMM_TC, NM_E_INVALID, "nm_gemm: bad backend");
   if (M == 0 || N == 0) return NM_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  const bool tc_ok = K > 0 && tc_gemm_supported(transA, transB, M, N, K, lda, ldb, ldc, A, B, C);
+  const bool tc_ok = K > 0 && tc_gemm_supported(M, N, K, lda, ldb, A, B);
   if (backend == NM_GEMM_TC)
     NM_REQUIRE(tc_ok, NM_E_UNSUPPORTED,
                "nm_gemm: shape not addressable by TMA (needs 16-byte aligned rows/pointers)");

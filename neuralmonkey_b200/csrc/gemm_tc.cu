@@ -574,17 +574,12 @@ __device__ __forceinline__ void load_mn_tile(uint8_t* __restrict__ dst, const Tc
 
 // ESZ = operand element size: 4 = fp32 consumed as TF32, 2 = fp16.  A k-block is 128 bytes of K either way
 // (32 or 64 elements) and one instruction consumes 32 of them, so the smem ring and the descriptors are the same.
-// PAIR: a cluster of two CTAs computes a 256 x BN tile (128 rows each) and shares its B tile: each CTA loads half
-// of every B k-block with a multicast TMA that lands in both CTAs, so a pair pulls B through L2 once instead of
-// twice.  A stage is refilled only when the consumers of BOTH CTAs have released it (their empty barriers count
-// the peer's warps too).  B must be K-major (TMA-loaded).
-template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ = 4, bool PAIR = false>
+template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                TcOperand opa, TcOperand opb, int64_t M, int64_t N, int64_t K, TcEpilogue epi, int splits,
                int kb_per_split, TcExt ext, TcBatch bt) {
   static_assert(ESZ == 2 || MODE != TC_EPI_XENT_BWD16, "the fp16 epilogue belongs to the fp16 instances");
-  static_assert(!PAIR || (!B_MN && BN % 16 == 0), "a pair multicasts whole 8-row swizzle atoms of a TMA-loaded B");
   constexpr int BK = 128 / ESZ;                // elements per 128-byte k-block
   constexpr bool MN16 = ESZ == 2 && A_MN && B_MN;   // fp16, both MN-major: TMA boxes, transposed wgmma operands
   constexpr bool A_MANUAL = A_MN && !MN16, B_MANUAL = B_MN && !MN16;
@@ -600,9 +595,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int TILE_M = PAIR ? 2 * TC_BM : TC_BM;
-  const uint32_t cta_rank = PAIR ? cluster_ctarank() : 0u;
-  const int64_t tiles_m = (M + TILE_M - 1) / TILE_M;
+  const int64_t tiles_m = (M + TC_BM - 1) / TC_BM;
   const int64_t tiles_n = (N + BN - 1) / BN;
   // split-K: the reduction is cut into `splits` slices, each an independent work item whose
   // epilogue adds its partial tile into C with red.global.add (weight-gradient products
@@ -610,7 +603,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   // batched: bt.count independent problems of this M x N x K, each a window of the operand tensors (no split-K)
   const bool batched = bt.count > 0;
   const int64_t tiles_per = tiles_m * tiles_n;
-  const int64_t tile = PAIR ? (int64_t)(blockIdx.x >> 1) : (int64_t)blockIdx.x;
+  const int64_t tile = blockIdx.x;
   const int64_t tm = tile % tiles_m, tn = (tile / tiles_m) % tiles_n;
   const int num_kb_total = (int)((K + BK - 1) / BK);  // host guarantees no empty split
   const int split = batched ? 0 : (int)(tile / tiles_per);
@@ -627,20 +620,19 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     b_row = prob_o * bt.b_row_outer + i * bt.b_row_inner;
     b_col = i * bt.b_col_inner;
   }
-  const int32_t m0 = (int32_t)(tm * TILE_M) + (int32_t)cta_rank * TC_BM, n0 = (int32_t)(tn * BN);
+  const int32_t m0 = (int32_t)(tm * TC_BM), n0 = (int32_t)(tn * BN);
 
   if (threadIdx.x == 0) {
     if (!A_MANUAL) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
     if (!B_MANUAL) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), MANUAL ? 128 : 1);
-      mbar_init(empty_bar(s), TC_EPI_WARPS * (PAIR ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
+      mbar_init(empty_bar(s), TC_EPI_WARPS);   // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers exist before anything arrives on them
   // Programmatic dependent launch (NMB200_TC_PDL): the barrier set-up above touches no global memory and may run
   // while the previous kernel of the stream drains; from here on its results are needed.  Without the launch
   // attribute both instructions do nothing.
@@ -653,8 +645,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     for (int kb = 0; kb < num_kb && (MANUAL || ptid == 0); ++kb) {
       const int s = kb % STAGES;
       const uint32_t phase = (uint32_t)((kb / STAGES) & 1);
-      if constexpr (PAIR) mbar_wait_cluster(empty_bar(s), phase ^ 1u);   // the peer's releases are cluster-scope
-      else mbar_wait(empty_bar(s), phase ^ 1u);
+      mbar_wait(empty_bar(s), phase ^ 1u);
       const uint32_t a_dst = smem_base + s * Cfg::STAGE_BYTES;
       const uint32_t b_dst = a_dst + TC_A_BYTES;
       const int32_t k0 = (kb_begin + kb) * BK;
@@ -671,10 +662,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         } else if (!A_MN) {
           tma_load_2d(a_dst, &map_a, full_bar(s), k0 + a_col, m0 + a_row);  // box {one k-block, 128 rows}
         }
-        if constexpr (PAIR) {   // this CTA's half of the B tile, into both CTAs
-          tma_load_2d_multicast(b_dst + cta_rank * (Cfg::B_BYTES / 2), &map_b, full_bar(s), k0 + b_col,
-                                n0 + b_row + (int32_t)cta_rank * (BN / 2), (uint16_t)3);
-        } else if (!B_MN) {   // (MN16 loaded it above)
+        if (!B_MN) {   // (MN16 loaded it above)
           tma_load_2d(b_dst, &map_b, full_bar(s), k0 + b_col, n0 + b_row);  // box {one k-block, BN rows}
         }
       }
@@ -708,10 +696,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     wgmma_commit();
     wgmma_wait<1>();                           // the previous k-block's products are done with their stage
     wgmma_fence_operands(acc);
-    if (prev_s >= 0 && lane == 0) {
-      mbar_arrive(empty_bar(prev_s));
-      if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(empty_bar(prev_s), cta_rank ^ 1u));   // the peer refills it too
-    }
+    if (prev_s >= 0 && lane == 0) mbar_arrive(empty_bar(prev_s));
     prev_s = s;
   }
   wgmma_wait<0>();
@@ -796,8 +781,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (MODE == TC_EPI_XENT_FWD && row < M)
     epi.part[(row * tiles_n + tn) * 2 + half] = make_float4(st.mx, st.sum, __int_as_float(st.arg), st.tgt);
   }
-  // a pair: neither CTA leaves while the other may still arrive on its barriers
-  if constexpr (PAIR) cluster_sync_all();
 }
 
 // ---------------------------------------------------------------------------
@@ -838,99 +821,6 @@ static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t c
   return NM_OK;
 }
 
-static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                      uint32_t box_rows);
-
-// One operand: a tensor map when it is K-major, the plain description the producer threads read otherwise.
-static int make_operand(CUtensorMap* map, TcOperand* op, bool mn_major, const void* base, int64_t rows, int64_t cols,
-                        int64_t ld, uint32_t box_rows, int esz) {
-  memset(map, 0, sizeof(*map));
-  *op = TcOperand{base, rows, cols, ld};
-  if (mn_major) return NM_OK;
-  if (esz == 4) return make_map(map, reinterpret_cast<const float*>(base), rows, cols, ld, box_rows);
-  return make_map16(map, base, rows, cols, ld, box_rows);
-}
-
-bool tc_gemm_supported(int transA, int transB, int64_t M, int64_t N, int64_t K, int64_t lda,
-                       int64_t ldb, int64_t ldc, const void* A, const void* B, const void* C) {
-  (void)transA; (void)transB; (void)ldc; (void)C;
-  if (M < 1 || N < 1 || K < 1) return false;
-  if ((lda & 3) || (ldb & 3)) return false;  // TMA global strides are multiples of 16 bytes
-  if (A && (reinterpret_cast<uintptr_t>(A) & 15)) return false;
-  if (B && (reinterpret_cast<uintptr_t>(B) & 15)) return false;
-  if (M > 0x7fffffffLL || N > 0x7fffffffLL || K > 0x7fffffffLL) return false;
-  return true;
-}
-
-// NMB200_TC_PDL=1: launch with programmatic stream serialization, so that a kernel's prologue overlaps the tail of
-// its predecessor (the kernel waits with griddepcontrol.wait before it touches global memory)
-static bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("NMB200_TC_PDL");
-    return e && atoi(e) != 0;
-  }();
-  return on;
-}
-
-// one CTA per work item (tile x split-K slice, or tile x batched problem); PAIR: a cluster of two CTAs per
-// 256-row work item
-template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ, bool PAIR = false>
-static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
-                        int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, int splits, int kb_per_split,
-                        const TcExt& ext, const TcBatch& bt, cudaStream_t s, const char* name) {
-  using Cfg = TcCfg<BN>;
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE, ESZ, PAIR>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_done = true;
-  }
-  const int64_t items = ceil_div(M, PAIR ? 2 * TC_BM : TC_BM) * ceil_div(N, BN) * (bt.count > 0 ? bt.count : splits);
-  NM_REQUIRE(items <= (PAIR ? 0x3fffffffLL : 0x7fffffffLL), NM_E_INVALID, "%s: %lld tiles", name, (long long)items);
-  if (kb_per_split <= 0) kb_per_split = (int)ceil_div(K, 128 / ESZ);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(PAIR ? 2 * items : items));
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = (size_t)Cfg::SMEM_BYTES;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[2];
-  int nattr = 0;
-  if (PAIR) {
-    attr[nattr].id = cudaLaunchAttributeClusterDimension;
-    attr[nattr].val.clusterDim.x = 2;
-    attr[nattr].val.clusterDim.y = 1;
-    attr[nattr].val.clusterDim.z = 1;
-    ++nattr;
-  }
-  if (pdl_enabled()) {
-    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[nattr].val.programmaticStreamSerializationAllowed = 1;
-    ++nattr;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = nattr;
-  NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt));
-  NM_LAUNCH_CHECK(name);
-  return NM_OK;
-}
-
-template <int BN, bool A_MN, bool B_MN, int MODE, bool PAIR = false>
-static int launch_cfg(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
-                      int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, cudaStream_t s, int splits = 1,
-                      int kb_per_split = 0) {
-  return launch_tiles<BN, A_MN, B_MN, MODE, 4, PAIR>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, TcExt{},
-                                               TcBatch{}, s, "tc_gemm_kernel");
-}
-
-// fp16 operands: no split-K.  MN = both operands MN-major (the reduction dimension strided: X^T . dY products),
-// otherwise both K-major.
-template <int BN, int MODE, bool MN = false, bool PAIR = false>
-static int launch_cfg16(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
-                        int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
-  return launch_tiles<BN, MN, MN, MODE, 2, PAIR>(ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
-                                           "tc_gemm_kernel(fp16)");
-}
-
 // 2-D fp16 tensor [rows, cols] with row pitch ld (elements), K-major operand tile: box = {64 elements of K,
 // box_rows}, 128-byte swizzle.
 static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
@@ -950,11 +840,99 @@ static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t 
   return NM_OK;
 }
 
-template <int BN, bool A_MN, bool B_MN, int MODE>
-static int launch_batched(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
-                          int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, const TcBatch& bt, cudaStream_t s) {
-  return launch_tiles<BN, A_MN, B_MN, MODE, 4>(ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s,
-                                               "tc_gemm_kernel(batched)");
+// One operand: a tensor map when it is K-major, the plain description the producer threads read otherwise.
+static int make_operand(CUtensorMap* map, TcOperand* op, bool mn_major, const void* base, int64_t rows, int64_t cols,
+                        int64_t ld, uint32_t box_rows, int esz) {
+  memset(map, 0, sizeof(*map));
+  *op = TcOperand{base, rows, cols, ld};
+  if (mn_major) return NM_OK;
+  if (esz == 4) return make_map(map, reinterpret_cast<const float*>(base), rows, cols, ld, box_rows);
+  return make_map16(map, base, rows, cols, ld, box_rows);
+}
+
+bool tc_gemm_supported(int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, const void* A, const void* B) {
+  if (M < 1 || N < 1 || K < 1) return false;
+  if ((lda & 3) || (ldb & 3)) return false;  // TMA global strides are multiples of 16 bytes
+  if (A && (reinterpret_cast<uintptr_t>(A) & 15)) return false;
+  if (B && (reinterpret_cast<uintptr_t>(B) & 15)) return false;
+  if (M > 0x7fffffffLL || N > 0x7fffffffLL || K > 0x7fffffffLL) return false;
+  return true;
+}
+
+// NMB200_TC_PDL=1: launch with programmatic stream serialization, so that a kernel's prologue overlaps the tail of
+// its predecessor (the kernel waits with griddepcontrol.wait before it touches global memory)
+static bool pdl_enabled() {
+  static const bool on = [] {
+    const char* e = getenv("NMB200_TC_PDL");
+    return e && atoi(e) != 0;
+  }();
+  return on;
+}
+
+// one CTA per work item (tile x split-K slice, or tile x batched problem)
+template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ>
+static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                        int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, int splits, int kb_per_split,
+                        const TcExt& ext, const TcBatch& bt, cudaStream_t s, const char* name) {
+  using Cfg = TcCfg<BN>;
+  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, MODE, ESZ>;
+  static bool attr_done = false;
+  if (!attr_done) {
+    NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    attr_done = true;
+  }
+  const int64_t items = ceil_div(M, TC_BM) * ceil_div(N, BN) * (bt.count > 0 ? bt.count : splits);
+  NM_REQUIRE(items <= 0x7fffffffLL, NM_E_INVALID, "%s: %lld tiles", name, (long long)items);
+  if (kb_per_split <= 0) kb_per_split = (int)ceil_div(K, 128 / ESZ);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)items);
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = (size_t)Cfg::SMEM_BYTES;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  if (pdl_enabled()) {
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+  }
+  NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt));
+  NM_LAUNCH_CHECK(name);
+  return NM_OK;
+}
+
+// launch_tiles for the tile width bn.  Only the widths each kind of product uses are instantiated: dense products
+// 64, 128, 160 and 256 columns (fp16 with both operands MN-major: no 160), the vocabulary cross-entropy
+// TC_XENT_BN, the attention epilogues 128.
+template <bool A_MN, bool B_MN, int MODE, int ESZ>
+static int launch_bn(int bn, const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
+                     int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, int splits, int kb_per_split,
+                     const TcExt& ext, const TcBatch& bt, cudaStream_t s, const char* name) {
+  constexpr bool dense = MODE == TC_EPI_DENSE, attn = MODE == TC_EPI_SOFTMAX || MODE == TC_EPI_DSOFTMAX;
+  switch (bn) {
+    case 64:
+      if constexpr (dense)
+        return launch_tiles<64, A_MN, B_MN, MODE, ESZ>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt,
+                                                       s, name);
+      break;
+    case 128:
+      if constexpr (dense || attn)
+        return launch_tiles<128, A_MN, B_MN, MODE, ESZ>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt,
+                                                        s, name);
+      break;
+    case 160:
+      if constexpr (dense && !(ESZ == 2 && A_MN))
+        return launch_tiles<160, A_MN, B_MN, MODE, ESZ>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt,
+                                                        s, name);
+      break;
+    case 256:
+      if constexpr (!attn)
+        return launch_tiles<256, A_MN, B_MN, MODE, ESZ>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt,
+                                                        s, name);
+      break;
+  }
+  set_error("%s: no instance with %d-column tiles for epilogue %d", name, bn, MODE);
+  return NM_E_UNSUPPORTED;
 }
 
 int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t a_rows,
@@ -980,47 +958,18 @@ int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t
   if (rc) return rc;
   rc = make_operand(&mb, &ob, b_mn, B, b_rows, b_cols, ldb, (uint32_t)bn, 4);
   if (rc) return rc;
+  const char* name = "tc_gemm_kernel(batched)";
   if (epi.mode == TC_EPI_SOFTMAX)
-    return launch_batched<128, false, false, TC_EPI_SOFTMAX>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+    return launch_bn<false, false, TC_EPI_SOFTMAX, 4>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s, name);
   if (epi.mode == TC_EPI_DSOFTMAX)
-    return launch_batched<128, false, false, TC_EPI_DSOFTMAX>(ma, mb, oa, ob, M, N, K, epi, bt, s);
+    return launch_bn<false, false, TC_EPI_DSOFTMAX, 4>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s, name);
   NM_REQUIRE(b_mn, NM_E_UNSUPPORTED, "tc_gemm_batched: dense products take an MN-major B operand");
-  if (bn == 64) {
-    if (a_mn) return launch_batched<64, true, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
-    return launch_batched<64, false, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
-  }
-  if (a_mn) return launch_batched<128, true, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
-  return launch_batched<128, false, true, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, bt, s);
-}
-
-// CTA pairs (tc_gemm_set_pair_mode): 0 = never, 1 = wherever the shape allows, -1 = the library's policy, which
-// is one CTA per tile (pairs are not measured to be faster on any product of the workloads).  NMB200_TC_PAIR
-// presets the mode.
-static int g_pair_override = -2;   // -2 = not set
-static int pair_mode() {
-  static const int mode = [] {
-    const char* e = getenv("NMB200_TC_PAIR");
-    return (e && *e) ? atoi(e) : -1;
-  }();
-  return g_pair_override != -2 ? g_pair_override : mode;
-}
-int tc_gemm_set_pair_mode(int mode) {
-  const int before = pair_mode();
-  g_pair_override = mode;
-  return before;
-}
-// a pair shares a TMA-loaded (K-major) B tile of 128 or 256 columns between two 128-row halves
-static bool pair_wanted(int64_t M, int bn, bool b_tma) {
-  return pair_mode() == 1 && b_tma && (bn == 128 || bn == 256) && M > TC_BM;
+  if (a_mn)
+    return launch_bn<true, true, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s, name);
+  return launch_bn<false, true, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s, name);
 }
 
 static int pick_bn(int64_t M, int64_t N, int64_t K) {
-  static const int forced = [] {   // NMB200_TC_BN={64,128,160,256}: tile-width experiments (tools/gemm_sweep.py)
-    const char* e = getenv("NMB200_TC_BN");
-    const int v = e ? atoi(e) : 0;
-    return (v == 64 || v == 128 || v == 160 || v == 256) ? v : 0;
-  }();
-  if (forced) return forced;
   if (N <= 64) return 64;
   if (N <= 128) return 128;
   // skinny output, very long reduction (dX of the vocabulary projection: 12800 x 300 x 32000):
@@ -1074,55 +1023,57 @@ int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, cons
   TcOperand oa, ob;
   int rc = a_mn ? make_operand(&ma, &oa, true, A, K, M, lda, TC_BM, 4) : make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 4);
   if (rc) return rc;
-  const bool pair = pair_wanted(M, bn, !b_mn);
   rc = b_mn ? make_operand(&mb, &ob, true, B, K, N, ldb, (uint32_t)bn, 4)
-            : make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)(pair ? bn / 2 : bn), 4);
+            : make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)bn, 4);
   if (rc) return rc;
   if (splits > 1 && epi.beta == 0.f)  // partial sums are added: start from zero
     NM_CUDA_TRY(cudaMemset2DAsync(epi.C, sizeof(float) * epi.ldc, 0, sizeof(float) * N, M, s));
-#define NM_TC_DISPATCH(BN_, MODE_)                                                                               \
-  do {                                                                                                           \
-    if (!a_mn && !b_mn) return launch_cfg<BN_, false, false, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per); \
-    if (!a_mn && b_mn) return launch_cfg<BN_, false, true, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);   \
-    if (a_mn && !b_mn) return launch_cfg<BN_, true, false, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);   \
-    return launch_cfg<BN_, true, true, MODE_>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);                       \
-  } while (0)
-  if (pair) {   // B K-major
-    if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg<256, false, false, TC_EPI_XENT_FWD, true>(ma, mb, oa, ob, M, N, K, epi, s);
-    if (epi.mode == TC_EPI_XENT_BWD) return launch_cfg<256, false, false, TC_EPI_XENT_BWD, true>(ma, mb, oa, ob, M, N, K, epi, s);
-    if (bn == 128) {
-      if (a_mn) return launch_cfg<128, true, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
-      return launch_cfg<128, false, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
-    }
-    if (a_mn) return launch_cfg<256, true, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
-    return launch_cfg<256, false, false, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, s, splits, kb_per);
-  }
-  if (epi.mode == TC_EPI_XENT_FWD) {  // A is always K-major for the vocabulary projection
-    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, s);
-    return launch_cfg<256, false, false, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, s);
+  const TcExt ext{};
+  const TcBatch bt{};
+  const char* name = "tc_gemm_kernel";
+  // A is always K-major for the vocabulary projection
+  if (epi.mode == TC_EPI_XENT_FWD) {
+    if (b_mn)
+      return launch_bn<false, true, TC_EPI_XENT_FWD, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s,
+                                                        name);
+    return launch_bn<false, false, TC_EPI_XENT_FWD, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s,
+                                                       name);
   }
   if (epi.mode == TC_EPI_XENT_BWD) {
-    if (b_mn) return launch_cfg<256, false, true, TC_EPI_XENT_BWD>(ma, mb, oa, ob, M, N, K, epi, s);
-    return launch_cfg<256, false, false, TC_EPI_XENT_BWD>(ma, mb, oa, ob, M, N, K, epi, s);
+    if (b_mn)
+      return launch_bn<false, true, TC_EPI_XENT_BWD, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s,
+                                                        name);
+    return launch_bn<false, false, TC_EPI_XENT_BWD, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s,
+                                                       name);
   }
-  if (bn == 64) NM_TC_DISPATCH(64, TC_EPI_DENSE);
-  if (bn == 128) NM_TC_DISPATCH(128, TC_EPI_DENSE);
-  if (bn == 160) NM_TC_DISPATCH(160, TC_EPI_DENSE);
-  NM_TC_DISPATCH(256, TC_EPI_DENSE);
-#undef NM_TC_DISPATCH
+  if (!a_mn && !b_mn)
+    return launch_bn<false, false, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s, name);
+  if (!a_mn)
+    return launch_bn<false, true, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s, name);
+  if (!b_mn)
+    return launch_bn<true, false, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s, name);
+  return launch_bn<true, true, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, splits, kb_per, ext, bt, s, name);
+}
+
+// fp16 operands: shapes within the kernel's 32-bit tile indices, 16-byte aligned bases and row pitches
+static int check_f16_operands(const char* name, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda,
+                              const void* B, int64_t ldb) {
+  NM_REQUIRE(M >= 1 && N >= 1 && K >= 1 && M <= 0x7fffffffLL && N <= 0x7fffffffLL && K <= 0x7fffffffLL,
+             NM_E_INVALID, "%s: bad shape %lld x %lld x %lld", name, (long long)M, (long long)N, (long long)K);
+  NM_REQUIRE((lda & 7) == 0 && (ldb & 7) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(B) & 15) == 0,
+             NM_E_INVALID, "%s: fp16 operands need 16-byte aligned bases and row pitches", name);
+  return NM_OK;
 }
 
 int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                         int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
   // A stored [K, M] (row pitch lda), B stored [K, N] (row pitch ldb): both MN-major
-  NM_REQUIRE(M >= 1 && N >= 1 && K >= 1 && M <= 0x7fffffffLL && N <= 0x7fffffffLL && K <= 0x7fffffffLL,
-             NM_E_INVALID, "tc_gemm16_mn: bad shape %lld x %lld x %lld", (long long)M, (long long)N, (long long)K);
-  NM_REQUIRE((lda & 7) == 0 && (ldb & 7) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
-                 (reinterpret_cast<uintptr_t>(B) & 15) == 0,
-             NM_E_INVALID, "tc_gemm16_mn: fp16 operands need 16-byte aligned bases and row pitches");
+  int rc = check_f16_operands("tc_gemm16_mn", M, N, K, A, lda, B, ldb);
+  if (rc) return rc;
   NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16_mn: dense epilogue only");
   CUtensorMap ma, mb;   // [K, M] and [K, N] as stored, boxes of 64 columns x one 64-row k-block
-  int rc = make_map16(&ma, A, K, M, lda, 64);
+  rc = make_map16(&ma, A, K, M, lda, 64);
   if (rc) return rc;
   rc = make_map16(&mb, B, K, N, ldb, 64);
   if (rc) return rc;
@@ -1131,41 +1082,29 @@ int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t 
   if (N <= 64) bn = 64;
   else if (N <= 128) bn = 128;
   else if (ceil_div(M, TC_BM) * ceil_div(N, 256) < sm_count()) bn = 128;
-  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  return launch_cfg16<256, TC_EPI_DENSE, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  return launch_bn<true, true, TC_EPI_DENSE, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
+                                                "tc_gemm_kernel(fp16)");
 }
 
 int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
-  NM_REQUIRE(M >= 1 && N >= 1 && K >= 1 && M <= 0x7fffffffLL && N <= 0x7fffffffLL && K <= 0x7fffffffLL,
-             NM_E_INVALID, "tc_gemm16: bad shape %lld x %lld x %lld", (long long)M, (long long)N, (long long)K);
-  NM_REQUIRE((lda & 7) == 0 && (ldb & 7) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
-                 (reinterpret_cast<uintptr_t>(B) & 15) == 0,
-             NM_E_INVALID, "tc_gemm16: fp16 operands need 16-byte aligned bases and row pitches");
+  int rc = check_f16_operands("tc_gemm16", M, N, K, A, lda, B, ldb);
+  if (rc) return rc;
   const int bn = (epi.mode == TC_EPI_DENSE) ? pick_bn(M, N, K) : TC_XENT_BN;
   CUtensorMap ma, mb;
   TcOperand oa, ob;
-  int rc = make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 2);
+  rc = make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 2);
   if (rc) return rc;
-  const bool pair = pair_wanted(M, bn, true);
-  rc = make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)(pair ? bn / 2 : bn), 2);
+  rc = make_operand(&mb, &ob, false, B, N, K, ldb, (uint32_t)bn, 2);
   if (rc) return rc;
-  if (pair) {
-    if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg16<256, TC_EPI_XENT_FWD, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-    if (epi.mode == TC_EPI_XENT_BWD16)
-      return launch_cfg16<256, TC_EPI_XENT_BWD16, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-    NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16: unsupported epilogue %d", epi.mode);
-    if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-    return launch_cfg16<256, TC_EPI_DENSE, false, true>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  }
-  if (epi.mode == TC_EPI_XENT_FWD) return launch_cfg16<256, TC_EPI_XENT_FWD>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  if (epi.mode == TC_EPI_XENT_BWD16) return launch_cfg16<256, TC_EPI_XENT_BWD16>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  const char* name = "tc_gemm_kernel(fp16)";
+  if (epi.mode == TC_EPI_XENT_FWD)
+    return launch_bn<false, false, TC_EPI_XENT_FWD, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s, name);
+  if (epi.mode == TC_EPI_XENT_BWD16)
+    return launch_bn<false, false, TC_EPI_XENT_BWD16, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
+                                                         name);
   NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16: unsupported epilogue %d", epi.mode);
-  if (bn == 64) return launch_cfg16<64, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  if (bn == 128) return launch_cfg16<128, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  if (bn == 160) return launch_cfg16<160, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
-  return launch_cfg16<256, TC_EPI_DENSE>(ma, mb, oa, ob, M, N, K, epi, ext, s);
+  return launch_bn<false, false, TC_EPI_DENSE, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s, name);
 }
 
 }  // namespace nm

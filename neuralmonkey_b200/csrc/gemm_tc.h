@@ -74,8 +74,7 @@ int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t
                            int64_t ldb, const TcEpilogue& epi, const TcBatch& bt, cudaStream_t s);
 
 // True when the operands can be addressed by TMA (16-byte aligned rows and bases).
-bool tc_gemm_supported(int transA, int transB, int64_t M, int64_t N, int64_t K, int64_t lda,
-                       int64_t ldb, int64_t ldc, const void* A, const void* B, const void* C);
+bool tc_gemm_supported(int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, const void* A, const void* B);
 
 // op(A)[M,K] . op(B)[K,N] with the given epilogue.  Same operand conventions as nm_gemm.
 int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A,
@@ -91,10 +90,5 @@ int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda
 // [K,N] (row pitch ldb) - weight-gradient products X^T . dY without transposed copies.  Dense epilogue.
 int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                         int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s);
-
-// CTA pairs (a cluster of two CTAs per 256 x BN tile sharing a multicast B tile): -1 = the library's policy (one
-// CTA per tile), 0 = never, 1 = wherever the shape allows (B K-major, BN 128 or 256).  Returns the previous mode.
-// Overrides the NMB200_TC_PAIR environment variable.
-int tc_gemm_set_pair_mode(int mode);
 
 }  // namespace nm

@@ -64,7 +64,7 @@ int nm_logits_xent_fwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
   NM_REQUIRE(!logits_out || ldl >= V, NM_E_INVALID, "nm_logits_xent_fwd: ldl < V");
   NM_REQUIRE((reinterpret_cast<uintptr_t>(part) & 15) == 0, NM_E_INVALID,
              "nm_logits_xent_fwd: part must be 16-byte aligned");
-  NM_REQUIRE(tc_gemm_supported(0, transW, M, V, K, ldx, ldw, V, X, W, nullptr), NM_E_UNSUPPORTED,
+  NM_REQUIRE(tc_gemm_supported(M, V, K, ldx, ldw, X, W), NM_E_UNSUPPORTED,
              "nm_logits_xent_fwd: operands not TMA-addressable (use nm_gemm + nm_xent_fwd)");
   cudaStream_t s = (cudaStream_t)stream;
   TcEpilogue epi{};
@@ -93,7 +93,7 @@ int nm_logits_xent_bwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
              "nm_logits_xent_bwd: null pointer");
   NM_REQUIRE(M > 0 && V > 0 && K > 0 && ldx >= K && ldw >= (transW ? K : V) && ldd >= V, NM_E_INVALID,
              "nm_logits_xent_bwd: bad sizes");
-  NM_REQUIRE(tc_gemm_supported(0, transW, M, V, K, ldx, ldw, ldd, X, W, dlogits), NM_E_UNSUPPORTED,
+  NM_REQUIRE(tc_gemm_supported(M, V, K, ldx, ldw, X, W), NM_E_UNSUPPORTED,
              "nm_logits_xent_bwd: operands not TMA-addressable (use nm_gemm + nm_xent_bwd)");
   TcEpilogue epi{};
   epi.mode = TC_EPI_XENT_BWD;

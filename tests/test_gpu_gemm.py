@@ -27,6 +27,9 @@ def _ref(a, b, ta, tb):
 @pytest.mark.parametrize("tb", [False, True])
 @pytest.mark.parametrize("shape", [(128, 128, 32), (256, 384, 96), (200, 300, 300), (1000, 600, 300),
                                    (12, 900, 1200), (300, 1000, 1024), (129, 257, 36),
+                                   (256, 128, 32), (512, 384, 96), (257, 260, 36), (4096, 512, 512),
+                                   (640, 2048, 200), (300, 600, 12800),
+                                   (8192, 1024, 64),     # enough tiles for 256-wide ones
                                    (1100, 300, 8192)])   # skinny N, long K: 160-wide tiles (+ split-K)
 def test_tc_gemm_matches_fp64(ta, tb, shape):
     from neuralmonkey_b200 import lib, ops

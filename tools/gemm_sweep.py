@@ -151,7 +151,6 @@ def main():
     groups = {"ende": ENDE_MN if args.kmajor else ENDE, "transformer": TRANSFORMER_MN if args.kmajor else TRANSFORMER,
               "diag": [] if args.kmajor else DIAG}
     shapes = [(g,) + s for g in ("ende", "transformer", "diag") if args.set in (g, "all") for s in groups[g]]
-    print("NMB200_TC_BN =", os.environ.get("NMB200_TC_BN", "(auto)"))
     for group, label, ta, tb, m, n, k in shapes:
         flop = 2.0 * m * n * k
         head = "{:12s} {} {:6d} x {:5d} x {:6d}".format(group, label, m, n, k)
