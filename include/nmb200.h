@@ -460,14 +460,6 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
 /* Diagnostic: 8 int64 device counters receiving the cycle counter of CTA 0 at the phase boundaries of the
  * following nm_attn_decoder_step_fwd launches; NULL switches it off. */
 int nm_attn_decoder_step_debug(void* counters);
-/* Where the step kernel takes its weight slices from: 1 = staged through shared memory as 2-D TMA tiles (one
- * elected thread, an mbarrier ring running ahead across the phases of the step), 0 = 16-byte loads from L2,
- * -1 = the library's default (NMB200_DECSTEP_WTMA presets it).  Same arithmetic in the same order either way. */
-int nm_attn_decoder_step_set_staging(int mode);
-/* Hypotheses a cluster of the step kernel owns: 8, or 16 (every weight byte a cluster pulls from L2 then feeds
- * twice the rows and half as many clusters re-read the weights; needs the 16-byte path), -1 = the library's default
- * (NMB200_DECSTEP_ROWS presets it). */
-int nm_attn_decoder_step_set_rows(int rows);
 
 /* ---- K5/K6 at run time: logits, argmax and the symbol bookkeeping of one decoding step ------
  * Replaces get_body of decoders/autoregressive.py:446-480 after next_state: logits = X.W + b

@@ -36,22 +36,16 @@ namespace cg = cooperative_groups;
 
 namespace nm {
 
-constexpr int DS_R = 8;          // rows per cluster (the default; DS_R_MAX with NMB200_DECSTEP_ROWS=16)
-constexpr int DS_R_MAX = 16;     // 16 rows per cluster: every weight byte a cluster pulls from L2 feeds twice the rows
+constexpr int DS_R = 8;          // rows (hypotheses) per cluster
 constexpr int DS_THREADS = 512;
 constexpr int DS_WARPS = DS_THREADS / 32;
 constexpr int DS_UNROLL = 8;     // weight rows in flight per thread
 constexpr int DS_SLOTS = 4;      // TMA ring depth
 constexpr int DS_RED_FLOATS = 128 * 32;   // K-split scratch of ds_panel: up to 128 partial sums of 32 floats
-constexpr int DS_WSLOTS = 4;     // weight-tile ring depth (weights staged by 2-D TMA)
-constexpr int DS_WKT = 32;       // weight rows (k) per staged tile
-constexpr int DS_WTMA_DEFAULT = 0;   // measured slower than the 16-byte loads (DESIGN.md): NMB200_DECSTEP_WTMA=1 opts in
-constexpr int DS_ROWS_DEFAULT = 8;   // 16 measured slower (16 clusters of 8 CTAs do not fit the chip at once: DESIGN.md)
 
 struct DecStep {
   int rows, E, H, A, C, Tx, O, group, act, maxout;
   int cl;            // cluster size
-  int R;             // rows (hypotheses) per cluster: 8 or 16
   int tck, tcv;      // time steps per staged keys / values tile (TMA path)
   int slot_floats;   // floats per ring slot (TMA path)
   const int64_t* symbols;
@@ -64,16 +58,11 @@ struct DecStep {
   const float *Wo, *bo;
   float *x_out, *h_out, *ctx_out, *w_out, *out;
   long long* prof;   // diagnostic: 8 clock64 stamps of CTA 0 (phase boundaries), or null
-  // weights staged through shared memory by 2-D TMA (wtma = 1): one tensor map per weight matrix
-  // (gates, candidate, query, output), box = {wbox[m] columns, DS_WKT rows}
-  int wtma, wslot_floats;
-  int wbox[4];
-  alignas(64) CUtensorMap wmap[4];
 };
 
 // Shared-memory carve-up (float offsets), the same arithmetic on host and device.
 struct DsLayout {
-  int xT, hT, rhT, hnT, ctxT, ug, res, red, qs, es, vs, ring, bars, wring, wbars, total;
+  int xT, hT, rhT, hnT, ctxT, ug, res, red, qs, es, vs, ring, bars, total;
   int res_ld;
 };
 
@@ -81,29 +70,26 @@ __host__ __device__ inline int ds_align4(int x) { return (x + 3) & ~3; }
 
 __host__ __device__ inline DsLayout ds_layout(const DecStep& p, bool tma) {
   DsLayout L;
-  const int rpc = p.R / p.cl;
+  const int rpc = DS_R / p.cl;
   int maxn = 2 * p.H;
   if (p.A > maxn) maxn = p.A;
   const int no = (p.maxout ? 2 : 1) * p.O;
   if (no > maxn) maxn = no;
   L.res_ld = ds_align4((maxn + p.cl - 1) / p.cl + 16);
   int o = 0;
-  L.xT = o;   o += ds_align4(p.E * p.R);
-  L.hT = o;   o += ds_align4(p.H * p.R);
-  L.rhT = o;  o += ds_align4(p.H * p.R);
-  L.hnT = o;  o += ds_align4(p.H * p.R);
-  L.ctxT = o; o += ds_align4(p.C * p.R);
-  L.ug = o;   o += ds_align4(p.R * ((p.H + p.cl - 1) / p.cl + 8));
-  L.res = o;  o += p.R * L.res_ld;
+  L.xT = o;   o += ds_align4(p.E * DS_R);
+  L.hT = o;   o += ds_align4(p.H * DS_R);
+  L.rhT = o;  o += ds_align4(p.H * DS_R);
+  L.hnT = o;  o += ds_align4(p.H * DS_R);
+  L.ctxT = o; o += ds_align4(p.C * DS_R);
+  L.ug = o;   o += ds_align4(DS_R * ((p.H + p.cl - 1) / p.cl + 8));
+  L.res = o;  o += DS_R * L.res_ld;
   L.red = o;  o += DS_RED_FLOATS;
   L.qs = o;   o += ds_align4(rpc * p.A);
   L.es = o;   o += ds_align4(rpc * p.Tx);
   L.vs = o;   o += ds_align4(p.A);
   L.ring = o; o += tma ? DS_SLOTS * p.slot_floats : 0;
   L.bars = o; o += 4 * DS_SLOTS;            // DS_SLOTS mbarriers (8 bytes each) + padding
-  o = (o + 31) & ~31;                       // TMA destinations: 128-byte aligned
-  L.wring = o; o += p.wtma ? DS_WSLOTS * p.wslot_floats : 0;
-  L.wbars = o; o += p.wtma ? 4 * DS_WSLOTS : 0;   // full[DS_WSLOTS] | empty[DS_WSLOTS]
   L.total = o;
   return L;
 }
@@ -164,13 +150,12 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   return v;
 }
 
-template <int G, int R>
+template <int G>
 __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const float* __restrict__ W,
                                       int ldw, int colA, int nA, int colB, int nB,
                                       float* __restrict__ res, int res_ld, float* __restrict__ red) {
   const int ng = nA + nB;
-  constexpr int RG = R * G;
-  constexpr int UN = R > 8 ? DS_UNROLL / 2 : DS_UNROLL;   // weight rows in flight per thread
+  constexpr int RG = DS_R * G;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // groups per warp: the choice that keeps most warps busy (38 groups: gw = 8 -> 5 quads x 3 warps; gw = 4
   // would leave 6 of 16 warps idle and every busy lane with twice the k range)
@@ -198,9 +183,9 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
     const int kper = (K + kslices - 1) / kslices;
     const int k0 = min(K, (ws * DS_KSL + ksl) * kper);
     const int k1 = min(K, k0 + kper);
-    float acc[R][G];
+    float acc[DS_R][G];
 #pragma unroll
-    for (int r = 0; r < R; ++r)
+    for (int r = 0; r < DS_R; ++r)
 #pragma unroll
       for (int c = 0; c < G; ++c) acc[r][c] = 0.f;
     if (active) {
@@ -211,14 +196,14 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
         const int lo = max(k0, start), hi = min(k1, start + len);
         if (lo < hi) {
           const float* wp = W + (int64_t)lo * ldw + col;
-          uint32_t ip = smem_u32(segs[s].inT) + (uint32_t)(lo - start) * R * 4u;
+          uint32_t ip = smem_u32(segs[s].inT) + (uint32_t)(lo - start) * DS_R * 4u;
           // batches of DS_UNROLL weight rows: all loads of a batch are in flight together; the last,
           // partial batch is predicated instead of falling back to one dependent load per row
 #pragma unroll 1
-          for (int k = lo; k < hi; k += UN) {
-            float w[UN][G];
+          for (int k = lo; k < hi; k += DS_UNROLL) {
+            float w[DS_UNROLL][G];
 #pragma unroll
-            for (int u = 0; u < UN; ++u) {
+            for (int u = 0; u < DS_UNROLL; ++u) {
               if (k + u < hi) {
                 if constexpr (G == 4) {
                   const float4 t = ldg_weight4(wp + (int64_t)u * ldw, wpolicy);
@@ -232,22 +217,22 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
               }
             }
 #pragma unroll
-            for (int u = 0; u < UN; ++u) {
+            for (int u = 0; u < DS_UNROLL; ++u) {
               if (k + u < hi) {
-                float in[R];
+                float in[DS_R];
 #pragma unroll
-                for (int q = 0; q < R / 4; ++q) {
-                  const float4 t4 = lds128(ip + u * R * 4 + 16 * q);
+                for (int q = 0; q < DS_R / 4; ++q) {
+                  const float4 t4 = lds128(ip + u * DS_R * 4 + 16 * q);
                   in[4 * q] = t4.x; in[4 * q + 1] = t4.y; in[4 * q + 2] = t4.z; in[4 * q + 3] = t4.w;
                 }
 #pragma unroll
-                for (int r = 0; r < R; ++r)
+                for (int r = 0; r < DS_R; ++r)
 #pragma unroll
                   for (int c = 0; c < G; ++c) acc[r][c] = fmaf(in[r], w[u][c], acc[r][c]);
               }
             }
-            wp += (int64_t)UN * ldw;
-            ip += UN * R * 4;
+            wp += (int64_t)DS_UNROLL * ldw;
+            ip += DS_UNROLL * DS_R * 4;
           }
         }
         start += len;
@@ -258,7 +243,7 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
     for (int off = 2; off < 32; off <<= 1) {
       if (off >= DS_GW) {        // warp-uniform
 #pragma unroll
-        for (int r = 0; r < R; ++r)
+        for (int r = 0; r < DS_R; ++r)
 #pragma unroll
           for (int c = 0; c < G; ++c) acc[r][c] += __shfl_xor_sync(0xffffffffu, acc[r][c], off);
       }
@@ -266,7 +251,7 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
     if (wsplit == 1) {
       if (active && ksl == 0) {
 #pragma unroll
-        for (int r = 0; r < R; ++r)
+        for (int r = 0; r < DS_R; ++r)
 #pragma unroll
           for (int c = 0; c < G; ++c) res[r * res_ld + gg * G + c] = acc[r][c];
       }
@@ -276,7 +261,7 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
       if (ws < wsplit && ksl == 0) {
         const int slot = ws * nq * DS_GW + quad * DS_GW + gl;
 #pragma unroll
-        for (int r = 0; r < R; ++r)
+        for (int r = 0; r < DS_R; ++r)
 #pragma unroll
           for (int c = 0; c < G; ++c) red[(r * G + c) * S + slot] = acc[r][c];
       }
@@ -297,151 +282,6 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
   }
 }
 
-// ---- weights through shared memory ------------------------------------------------------------------------
-// The loop above keeps 8 independent 16-byte loads per thread in flight, yet a CTA pulls its weight slice at a
-// tenth of the rate one SM can take from L2 (ncu: long-scoreboard stalls; the load/store path tracks far fewer
-// requests than 512 threads can issue).  Here the slice arrives as 2-D TMA tiles - DS_WKT weight rows by the
-// CTA's column range(s), one elected thread, a DS_WSLOTS-deep mbarrier ring running ahead ACROSS the phases
-// (the first tiles of the next product stream in while this one is reduced and the cluster synchronises) - and
-// the FMA loop reads weights and inputs from shared memory.  Thread mapping and reduction are those of ds_panel,
-// with the k rows of a column group dealt round-robin to its lanes so that every tile feeds all lanes.
-struct DsWPanel {
-  int map, K, colA, colB, nbox, bc, ntiles, tile0;
-};
-struct DsWSched {
-  int issued, total;
-  DsWPanel pan[4];
-};
-
-__device__ __forceinline__ void ds_w_refill(const DecStep& p, DsWSched& S, int upto, uint32_t wring_u32,
-                                            uint32_t wbar) {   // thread 0
-  while (S.issued < S.total && S.issued < upto) {
-    const int j = S.issued;
-    int pi = 0;
-    while (pi < 3 && j >= S.pan[pi].tile0 + S.pan[pi].ntiles) ++pi;
-    const DsWPanel& w = S.pan[pi];
-    const int kt = j - w.tile0, slot = j % DS_WSLOTS;
-    if (j >= DS_WSLOTS) mbar_wait(wbar + 8u * (DS_WSLOTS + slot), (uint32_t)(((j / DS_WSLOTS) - 1) & 1));
-    const uint32_t box_bytes = (uint32_t)(DS_WKT * w.bc * 4);
-    mbar_expect_tx(wbar + 8u * slot, box_bytes * (uint32_t)w.nbox);
-    const uint32_t dst = wring_u32 + (uint32_t)(slot * p.wslot_floats * 4);
-    tma_load_2d(dst, &p.wmap[w.map], wbar + 8u * slot, w.colA, kt * DS_WKT);
-    if (w.nbox == 2) tma_load_2d(dst + box_bytes, &p.wmap[w.map], wbar + 8u * slot, w.colB, kt * DS_WKT);
-    ++S.issued;
-  }
-}
-
-__device__ __noinline__ void ds_panel_w(const DecStep& p, DsWSched& S, int pi, const DsSeg* segs, int nseg,
-                                        int nA, int nB, float* __restrict__ res, int res_ld,
-                                        float* __restrict__ red, const float* __restrict__ wring, uint32_t wbar) {
-  constexpr int G = 4;
-  constexpr int RG = DS_R * G;
-  const DsWPanel w = S.pan[pi];
-  const int ng = nA + nB, K = w.K;
-  if (ng <= 0) return;                                 // this CTA owns no column of the product (no tiles either)
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int DS_GW = DS_GW_MAX, best_busy = 0;
-#pragma unroll
-  for (int cand = 2; cand <= DS_GW_MAX; cand <<= 1) {
-    const int nqc = (ng + cand - 1) / cand;
-    if (nqc > DS_WARPS) continue;                      // one round: a tile is consumed once
-    const int busy = nqc * (DS_WARPS / nqc);
-    const bool fits = (DS_WARPS / nqc) == 1 || (DS_WARPS / nqc) * nqc * cand * RG <= DS_RED_FLOATS;
-    if (fits && (busy > best_busy || (busy == best_busy && cand == 4))) { best_busy = busy; DS_GW = cand; }
-  }
-  const int DS_KSL = 32 / DS_GW;
-  const int gl = lane % DS_GW, ksl = lane / DS_GW;
-  const int nq = (ng + DS_GW - 1) / DS_GW;             // <= DS_WARPS (host: ng <= DS_WARPS * DS_GW_MAX)
-  const int wsplit = nq > 0 ? DS_WARPS / nq : 1;
-  const int quad = nq > 0 ? warp % nq : 0, ws = nq > 0 ? warp / nq : DS_WARPS;
-  const int gg = quad * DS_GW + gl;
-  const bool active = ws < wsplit && gg < ng;
-  const int KS = DS_KSL * wsplit;                      // lanes sharing one column group (k rows dealt round-robin)
-  const int slice = ws * DS_KSL + ksl;
-  const int woff = gg < nA ? gg * G : DS_WKT * w.bc + (gg - nA) * G;
-  const int len0 = segs[0].len, len1 = nseg > 1 ? segs[1].len : 0;
-  const uint32_t in0 = smem_u32(segs[0].inT), in1 = nseg > 1 ? smem_u32(segs[1].inT) : 0u,
-                 in2 = nseg > 2 ? smem_u32(segs[2].inT) : 0u;
-  float acc[DS_R][G];
-#pragma unroll
-  for (int r = 0; r < DS_R; ++r)
-#pragma unroll
-    for (int c = 0; c < G; ++c) acc[r][c] = 0.f;
-  const uint32_t wring_u32 = smem_u32(wring);
-#pragma unroll 1
-  for (int tt = 0; tt < w.ntiles; ++tt) {
-    const int gi = w.tile0 + tt, slot = gi % DS_WSLOTS;
-    if (threadIdx.x == 0) ds_w_refill(p, S, gi + DS_WSLOTS, wring_u32, wbar);
-    mbar_wait(wbar + 8u * slot, (uint32_t)((gi / DS_WSLOTS) & 1));
-    if (active) {
-      const uint32_t wt = wring_u32 + (uint32_t)((slot * p.wslot_floats + woff) * 4);
-      const int k0 = tt * DS_WKT;
-#pragma unroll 4
-      for (int kk = slice; kk < DS_WKT; kk += KS) {
-        const int k = k0 + kk;
-        if (k < K) {
-          const float4 wv = lds128(wt + (uint32_t)(kk * w.bc * 4));
-          int ks = k;
-          uint32_t ib = in0;
-          if (nseg > 1 && ks >= len0) {
-            ks -= len0; ib = in1;
-            if (nseg > 2 && ks >= len1) { ks -= len1; ib = in2; }
-          }
-          const uint32_t ip = ib + (uint32_t)(ks * DS_R * 4);
-          const float4 i0 = lds128(ip), i1 = lds128(ip + 16);
-          const float in[DS_R] = {i0.x, i0.y, i0.z, i0.w, i1.x, i1.y, i1.z, i1.w};
-          const float wc[G] = {wv.x, wv.y, wv.z, wv.w};
-#pragma unroll
-          for (int r = 0; r < DS_R; ++r)
-#pragma unroll
-            for (int c = 0; c < G; ++c) acc[r][c] = fmaf(in[r], wc[c], acc[r][c]);
-        }
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(wbar + 8u * (DS_WSLOTS + slot));   // this warp is done with the slot
-  }
-  // the k-slices of a column group inside this warp: lanes gl, gl + gw, ...
-#pragma unroll
-  for (int off = 2; off < 32; off <<= 1) {
-    if (off >= DS_GW) {        // warp-uniform
-#pragma unroll
-      for (int r = 0; r < DS_R; ++r)
-#pragma unroll
-        for (int c = 0; c < G; ++c) acc[r][c] += __shfl_xor_sync(0xffffffffu, acc[r][c], off);
-    }
-  }
-  if (wsplit == 1) {
-    if (active && ksl == 0) {
-#pragma unroll
-      for (int r = 0; r < DS_R; ++r)
-#pragma unroll
-        for (int c = 0; c < G; ++c) res[r * res_ld + gg * G + c] = acc[r][c];
-    }
-  } else {
-    const int Sn = wsplit * nq * DS_GW;
-    if (ws < wsplit && ksl == 0) {
-      const int slotr = ws * nq * DS_GW + quad * DS_GW + gl;
-#pragma unroll
-      for (int r = 0; r < DS_R; ++r)
-#pragma unroll
-        for (int c = 0; c < G; ++c) red[(r * G + c) * Sn + slotr] = acc[r][c];
-    }
-    __syncthreads();
-#pragma unroll 1
-    for (int idx = threadIdx.x; idx < nq * DS_GW * RG; idx += DS_THREADS) {
-      const int e = idx / (nq * DS_GW), g2 = idx - e * (nq * DS_GW);
-      if (g2 < ng) {
-        float sum = 0.f;
-#pragma unroll 1
-        for (int h = 0; h < wsplit; ++h) sum += red[e * Sn + h * nq * DS_GW + g2];
-        res[(e / G) * res_ld + g2 * G + (e % G)] = sum;
-      }
-    }
-  }
-  __syncthreads();
-}
-
 // The slice of `total` G-wide groups CTA `rank` of `cl` owns: [first, first + count).
 __device__ __forceinline__ void ds_slice(int total, int cl, int rank, int& first, int& count) {
   const int per = (total + cl - 1) / cl;
@@ -453,19 +293,17 @@ __device__ __forceinline__ void ds_slice(int total, int cl, int rank, int& first
 // (a thread of the context pass owns one (row, column group) pair).  Computed by thread 0 into shared memory.
 struct DsRuns {
   int n;
-  int e[DS_R_MAX], first[DS_R_MAX], cnt[DS_R_MAX];
+  int e[DS_R], first[DS_R], cnt[DS_R];
 };
 
-template <int G, bool WT, int R>
+template <int G>
 __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const __grid_constant__ DecStep p) {
-  static_assert(!WT || G == 4, "staged weights need the 16-byte path");
-  static_assert(R == 8 || (R == DS_R_MAX && G == 4 && !WT), "16 rows per cluster: vector path, weights from L2");
   constexpr bool TMA = (G == 4);
   cg::cluster_group cluster = cg::this_cluster();
   const int CL = p.cl;
   const int rank = (int)cluster.block_rank();
-  const int row0 = (int)(blockIdx.x / CL) * R;
-  const int rpc = R / CL;                   // rows this CTA attends for
+  const int row0 = (int)(blockIdx.x / CL) * DS_R;
+  const int rpc = DS_R / CL;                // rows this CTA attends for
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const DsLayout L = ds_layout(p, TMA);
 
@@ -485,16 +323,13 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
   const uint32_t bar0 = smem_u32(smem + L.bars);
   const int res_ld = L.res_ld;
   __shared__ DsRuns runs;
-  __shared__ DsWSched wsched;
-  const float* wring = smem + L.wring;
-  const uint32_t wbar = smem_u32(smem + L.wbars);
 
   const int my0 = row0 + rank * rpc;                      // first global row this CTA attends for
   const int nmy = max(0, min(rpc, p.rows - my0));         // valid ones
   const int nk = TMA ? (p.Tx + p.tck - 1) / p.tck : 1;    // tiles per run: keys, then values
   const int nv = TMA ? (p.Tx + p.tcv - 1) / p.tcv : 1;
   const int ncg = (p.C + G - 1) / G;                      // context column groups (host: <= DS_THREADS)
-  const int jt = min(R, DS_THREADS / ncg);             // rows per run
+  const int jt = min(DS_R, DS_THREADS / ncg);          // rows per run
 
   // tile i of this CTA's schedule (run-major: the key tiles of a run, then its value tiles)
   auto issue_tile = [&](int i) {   // one thread
@@ -530,35 +365,11 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
       }
     }
     runs.n = n;
-    if (WT) {
-      // the weight tiles of this CTA, in the order the phases consume them
-      int uf2, un2, af2, an2, of2, on2;
-      ds_slice((p.H + 3) / 4, CL, rank, uf2, un2);
-      ds_slice((p.A + 3) / 4, CL, rank, af2, an2);
-      ds_slice((p.O + 3) / 4, CL, rank, of2, on2);
-      const int kin = p.E + p.H, kout = p.H + p.E + p.C;
-      wsched.pan[0] = DsWPanel{0, kin, uf2 * 4, p.H + uf2 * 4, 2, p.wbox[0], un2 > 0 ? (kin + DS_WKT - 1) / DS_WKT : 0, 0};
-      wsched.pan[1] = DsWPanel{1, kin, uf2 * 4, 0, 1, p.wbox[1], un2 > 0 ? (kin + DS_WKT - 1) / DS_WKT : 0, 0};
-      wsched.pan[2] = DsWPanel{2, p.H, af2 * 4, 0, 1, p.wbox[2], an2 > 0 ? (p.H + DS_WKT - 1) / DS_WKT : 0, 0};
-      wsched.pan[3] = DsWPanel{3, kout, of2 * 4, p.O + of2 * 4, p.maxout ? 2 : 1, p.wbox[3],
-                               on2 > 0 ? (kout + DS_WKT - 1) / DS_WKT : 0, 0};
-      int t0 = 0;
-#pragma unroll 1
-      for (int i = 0; i < 4; ++i) { wsched.pan[i].tile0 = t0; t0 += wsched.pan[i].ntiles; }
-      wsched.total = t0;
-      wsched.issued = 0;
-#pragma unroll 1
-      for (int s2 = 0; s2 < DS_WSLOTS; ++s2) {
-        mbar_init(wbar + 8u * s2, 1);
-        mbar_init(wbar + 8u * (DS_WSLOTS + s2), DS_WARPS);
-      }
-    }
     if (TMA) {
 #pragma unroll 1
       for (int s2 = 0; s2 < DS_SLOTS; ++s2) mbar_init(bar0 + 8u * s2, 1);
       asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      if (WT) ds_w_refill(p, wsched, DS_WSLOTS, smem_u32(wring), wbar);   // the first weight tiles stream in now
       const int first = min(n * (nk + nv), DS_SLOTS);
 #pragma unroll 1
       for (int i = 0; i < first; ++i) issue_tile(i);   // in flight while the GRU phases run
@@ -569,7 +380,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
   // lane -> (row = lane & 7, k offset = lane >> 3): the stores walk shared memory linearly (no bank
   // conflicts); the global side reads 16 contiguous bytes of each of the 8 rows per warp instruction
   {
-    const int r = lane & (R - 1);
+    const int r = lane & (DS_R - 1);
     const int grow = row0 + r;
     const bool ok = grow < p.rows;
     const float* xsrc = nullptr;
@@ -580,13 +391,13 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
       hsrc = p.h_prev + (int64_t)src * p.H;
     }
 #pragma unroll 1
-    for (int k = tid / R; k < p.E; k += DS_THREADS / R) {
+    for (int k = tid / DS_R; k < p.E; k += DS_THREADS / DS_R) {
       const float val = ok ? xsrc[k] : 0.f;
       if (ok && p.x_out && rank == 0) p.x_out[(int64_t)grow * p.E + k] = val;
-      xT[k * R + r] = val;
+      xT[k * DS_R + r] = val;
     }
 #pragma unroll 1
-    for (int k = tid / R; k < p.H; k += DS_THREADS / R) hT[k * R + r] = ok ? hsrc[k] : 0.f;
+    for (int k = tid / DS_R; k < p.H; k += DS_THREADS / DS_R) hT[k * DS_R + r] = ok ? hsrc[k] : 0.f;
   }
 #pragma unroll 1
   for (int a = tid; a < p.A; a += DS_THREADS) vs[a] = p.v[a];
@@ -596,8 +407,8 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
   cluster.sync();   // every CTA of the cluster has started: its shared memory may be written remotely
   if (prof) p.prof[1] = clock64();
 
-  const int r_w = warp & (R - 1), half_w = warp / R;   // element-wise passes: warp -> (row, half)
-  constexpr int NHALF = DS_WARPS / R;
+  const int r_w = warp & (DS_R - 1), half_w = warp / DS_R;   // element-wise passes: warp -> (row, half)
+  constexpr int NHALF = DS_WARPS / DS_R;
 
   // ---- phase 1: gates of this CTA's hidden units -------------------------------------------------
   int uf, un;   // first unit group / number of unit groups
@@ -606,17 +417,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
   const int nu = min(p.H, u0 + un * G) - u0;   // units this CTA owns (0 when H is small and CL large)
   {
     const DsSeg segs[2] = {{xT, p.E}, {hT, p.H}};
-    if constexpr (WT) ds_panel_w(p, wsched, 0, segs, 2, un, un, res, res_ld, red, wring, wbar);
-    else ds_panel<G, R>(segs, 2, p.E + p.H, p.Wg, 2 * p.H, u0, un, p.H + u0, un, res, res_ld, red);
+    ds_panel<G>(segs, 2, p.E + p.H, p.Wg, 2 * p.H, u0, un, p.H + u0, un, res, res_ld, red);
 #pragma unroll 1
     for (int ul = lane + 32 * half_w; ul < nu; ul += 32 * NHALF) {
       const int r = r_w, u = u0 + ul;
       const float rr = sigmoidf_(res[r * res_ld + ul] + p.bg[u]);
       const float uu = sigmoidf_(res[r * res_ld + un * G + ul] + p.bg[p.H + u]);
       ugs[r * nu + ul] = uu;
-      const float rh = rr * hT[u * R + r];
+      const float rh = rr * hT[u * DS_R + r];
 #pragma unroll 1
-      for (int c = 0; c < CL; ++c) cluster.map_shared_rank(rhT, c)[u * R + r] = rh;
+      for (int c = 0; c < CL; ++c) cluster.map_shared_rank(rhT, c)[u * DS_R + r] = rh;
     }
   }
   cluster.sync();
@@ -625,16 +435,15 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
   // ---- phase 2: candidate and new state ------------------------------------------------------------
   {
     const DsSeg segs[2] = {{xT, p.E}, {rhT, p.H}};
-    if constexpr (WT) ds_panel_w(p, wsched, 1, segs, 2, un, 0, res, res_ld, red, wring, wbar);
-    else ds_panel<G, R>(segs, 2, p.E + p.H, p.Wc, p.H, u0, un, 0, 0, res, res_ld, red);
+    ds_panel<G>(segs, 2, p.E + p.H, p.Wc, p.H, u0, un, 0, 0, res, res_ld, red);
 #pragma unroll 1
     for (int ul = lane + 32 * half_w; ul < nu; ul += 32 * NHALF) {
       const int r = r_w, u = u0 + ul;
       const float c = tanhf(res[r * res_ld + ul] + p.bc[u]);
       const float uu = ugs[r * nu + ul];
-      const float hn = uu * hT[u * R + r] + (1.f - uu) * c;
+      const float hn = uu * hT[u * DS_R + r] + (1.f - uu) * c;
 #pragma unroll 1
-      for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(hnT, cc)[u * R + r] = hn;
+      for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(hnT, cc)[u * DS_R + r] = hn;
       if (row0 + r < p.rows) p.h_out[(int64_t)(row0 + r) * p.H + u] = hn;
     }
   }
@@ -648,8 +457,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
     const int a0 = af * G;
     const int na = min(p.A, a0 + an * G) - a0;
     const DsSeg segs[1] = {{hnT, p.H}};
-    if constexpr (WT) ds_panel_w(p, wsched, 2, segs, 1, an, 0, res, res_ld, red, wring, wbar);
-    else ds_panel<G, R>(segs, 1, p.H, p.Wq, p.A, a0, an, 0, 0, res, res_ld, red);
+    ds_panel<G>(segs, 1, p.H, p.Wq, p.A, a0, an, 0, 0, res, res_ld, red);
     float* qdst = cluster.map_shared_rank(qs, r_w / rpc) + (r_w % rpc) * p.A;
 #pragma unroll 1
     for (int al = lane + 32 * half_w; al < na; al += 32 * NHALF)
@@ -785,7 +593,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
           const int col = cgi * G + c;
           if (col < p.C) {
 #pragma unroll 1
-            for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(ctxT, cc)[col * R + rl] = cacc[c];
+            for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(ctxT, cc)[col * DS_R + rl] = cacc[c];
             if (p.ctx_out) p.ctx_out[(int64_t)(my0 + j0 + cj) * p.C + col] = cacc[c];
           }
         }
@@ -798,7 +606,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
 #pragma unroll 1
       for (int col = tid; col < p.C; col += DS_THREADS)
 #pragma unroll 1
-        for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(ctxT, cc)[col * R + rl] = 0.f;
+        for (int cc = 0; cc < CL; ++cc) cluster.map_shared_rank(ctxT, cc)[col * DS_R + rl] = 0.f;
     }
   }
   if (prof) p.prof[5] = clock64();
@@ -813,8 +621,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
     const int no = min(p.O, o0 + on * G) - o0;
     const DsSeg segs[3] = {{hnT, p.H}, {xT, p.E}, {ctxT, p.C}};
     const int ldo = (p.maxout ? 2 : 1) * p.O;
-    if constexpr (WT) ds_panel_w(p, wsched, 3, segs, 3, on, p.maxout ? on : 0, res, res_ld, red, wring, wbar);
-    else ds_panel<G, R>(segs, 3, p.H + p.E + p.C, p.Wo, ldo, o0, on, p.O + o0, p.maxout ? on : 0, res, res_ld, red);
+    ds_panel<G>(segs, 3, p.H + p.E + p.C, p.Wo, ldo, o0, on, p.O + o0, p.maxout ? on : 0, res, res_ld, red);
     if (row0 + r_w < p.rows) {
 #pragma unroll 1
       for (int ol = lane + 32 * half_w; ol < no; ol += 32 * NHALF) {
@@ -838,54 +645,6 @@ __global__ void __launch_bounds__(DS_THREADS, 1) attn_decoder_step_kernel(const 
 using namespace nm;
 
 static long long* g_decstep_prof = nullptr;
-static int g_decstep_staging = -1;   // nm_attn_decoder_step_set_staging
-static int g_decstep_rows = -1;      // nm_attn_decoder_step_set_rows
-
-// 2-D tensor map of a row-major fp32 weight matrix [rows, cols]: box = {box_cols, DS_WKT rows}, no swizzle,
-// out-of-range elements read as zeros.  Encoded once per (matrix, box) and kept: the weights of a model do not move.
-namespace {
-typedef CUresult (*DsEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-struct DsMapKey {
-  const void* base;
-  int64_t rows, cols;
-  int box;
-  CUtensorMap map;
-};
-int ds_weight_map(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int box_cols) {
-  static DsMapKey cache[32];
-  static int used = 0, next = 0;
-  for (int i = 0; i < used; ++i)
-    if (cache[i].base == base && cache[i].rows == rows && cache[i].cols == cols && cache[i].box == box_cols) {
-      *out = cache[i].map;
-      return NM_OK;
-    }
-  static DsEncodeFn fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<DsEncodeFn>(ptr);
-  }
-  NM_REQUIRE(fn != nullptr, NM_E_NO_DEVICE, "nm_attn_decoder_step_fwd: cuTensorMapEncodeTiled not available");
-  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)cols * 4};
-  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)DS_WKT};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  NM_REQUIRE(r == CUDA_SUCCESS, NM_E_INVALID, "nm_attn_decoder_step_fwd: tensor map of a %lld x %lld weight failed (%d)",
-             (long long)rows, (long long)cols, (int)r);
-  DsMapKey& slot = cache[next];
-  slot.base = base; slot.rows = rows; slot.cols = cols; slot.box = box_cols; slot.map = *out;
-  next = (next + 1) % 32;
-  if (used < 32) ++used;
-  return NM_OK;
-}
-}  // namespace
 
 extern "C" {
 
@@ -894,18 +653,6 @@ extern "C" {
  * cluster joined | output done).  NULL = off. */
 int nm_attn_decoder_step_debug(void* counters) {
   g_decstep_prof = reinterpret_cast<long long*>(counters);
-  return NM_OK;
-}
-
-int nm_attn_decoder_step_set_staging(int mode) {
-  NM_REQUIRE(mode >= -1 && mode <= 1, NM_E_INVALID, "nm_attn_decoder_step_set_staging: mode must be -1, 0 or 1");
-  g_decstep_staging = mode;
-  return NM_OK;
-}
-
-int nm_attn_decoder_step_set_rows(int rows) {
-  NM_REQUIRE(rows == -1 || rows == 8 || rows == 16, NM_E_INVALID, "nm_attn_decoder_step_set_rows: -1, 8 or 16");
-  g_decstep_rows = rows;
   return NM_OK;
 }
 
@@ -943,67 +690,17 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
   NM_REQUIRE(ceil_div(C, g) <= DS_THREADS, NM_E_UNSUPPORTED,
              "nm_attn_decoder_step_fwd: context size %lld too large for one CTA", (long long)C);
 
-  // rows per cluster: 16 halves the number of clusters that re-read the weights (NMB200_DECSTEP_ROWS=8|16)
-  static const int rows_env = [] {
-    const char* e = getenv("NMB200_DECSTEP_ROWS");
-    const int v = (e && *e) ? atoi(e) : DS_ROWS_DEFAULT;
-    return v == 16 ? 16 : 8;
-  }();
-  const int rows_mode = g_decstep_rows > 0 ? g_decstep_rows : rows_env;
   // cluster size: as many CTAs as fill the chip, at most 8, at least one attended row per CTA
-  auto cluster_size = [&](int R) {
-    const int64_t n = ceil_div(rows, R);
-    int c = 8;
-    while (c > 1 && n * c > (int64_t)sm_count()) c >>= 1;
-    const char* env = getenv("NMB200_DECSTEP_CLUSTER");
-    if (env && *env) {
-      const int want = atoi(env);
-      if (want == 1 || want == 2 || want == 4 || want == 8) c = want;
-    }
-    return c;
-  };
-  p.R = (vec && rows_mode == 16 && rows > DS_R) ? DS_R_MAX : DS_R;
-  int cl = cluster_size(p.R);
-  if (p.R == DS_R_MAX) {   // twice the row vectors in shared memory: back to 8 rows when no key / value tile fits
-    DecStep q = p;
-    q.cl = cl;
-    q.slot_floats = 0;
-    const int64_t avail16 = (int64_t)(227 * 1024 - 1024) / 4 - ds_layout(q, true).total;
-    if (avail16 / DS_SLOTS - (avail16 / DS_SLOTS) % 32 < (A > C ? A : C)) {
-      p.R = DS_R;
-      cl = cluster_size(p.R);
-    }
+  const int64_t clusters = ceil_div(rows, DS_R);
+  int cl = 8;
+  while (cl > 1 && clusters * cl > (int64_t)sm_count()) cl >>= 1;
+  const char* env = getenv("NMB200_DECSTEP_CLUSTER");
+  if (env && *env) {
+    const int want = atoi(env);
+    if (want == 1 || want == 2 || want == 4 || want == 8) cl = want;
   }
-  const int64_t clusters = ceil_div(rows, p.R);
   p.cl = cl;
 
-  // weights through shared memory (2-D TMA tiles) when every column range fits one box; NMB200_DECSTEP_WTMA=0/1
-  static const int wtma_env = [] {
-    const char* e = getenv("NMB200_DECSTEP_WTMA");
-    return (e && *e) ? atoi(e) : DS_WTMA_DEFAULT;
-  }();
-  bool wt = vec && p.R == DS_R && (g_decstep_staging >= 0 ? g_decstep_staging : wtma_env) != 0;
-  if (wt) {
-    const int64_t totals[4] = {H / 4, H / 4, A / 4, O / 4};
-    const int nbox[4] = {2, 1, 1, maxout ? 2 : 1};
-    int64_t slot = 0;
-    for (int m = 0; m < 4 && wt; ++m) {
-      const int64_t per = ceil_div(totals[m], cl);
-      if (per * 4 > 256 || per > (int64_t)DS_WARPS * DS_GW_MAX / nbox[m]) wt = false;   // one box, one round
-      p.wbox[m] = (int)(per * 4);
-      const int64_t need = (int64_t)nbox[m] * DS_WKT * per * 4;
-      if (need > slot) slot = need;
-    }
-    if (wt) {
-      p.wslot_floats = (int)((slot + 31) / 32 * 32);
-      int rc = ds_weight_map(&p.wmap[0], Wg, E + H, 2 * H, p.wbox[0]);
-      if (!rc) rc = ds_weight_map(&p.wmap[1], Wc, E + H, H, p.wbox[1]);
-      if (!rc) rc = ds_weight_map(&p.wmap[2], Wq, H, A, p.wbox[2]);
-      if (!rc) rc = ds_weight_map(&p.wmap[3], Wo, H + E + C, (maxout ? 2 : 1) * O, p.wbox[3]);
-      if (rc) return rc;
-      p.wtma = 1;
-    }
-  }
   // ring slots: as large as the shared memory left over allows, whole time steps of keys / values
   size_t smem_bytes = 0;
   if (vec) {
@@ -1013,13 +710,6 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
     int64_t slot = avail / DS_SLOTS;
     slot -= slot % 32;                                       // 128-byte granularity
     const int64_t need = (A > C ? A : C);
-    if (slot < need && p.wtma) {   // the weight ring does not fit beside a key/value tile: stream weights from L2
-      p.wtma = 0;
-      p.wslot_floats = 0;
-      const DsLayout base2 = ds_layout(p, true);
-      slot = ((int64_t)(227 * 1024 - 1024) / 4 - base2.total) / DS_SLOTS;
-      slot -= slot % 32;
-    }
     NM_REQUIRE(slot >= need, NM_E_UNSUPPORTED,
                "nm_attn_decoder_step_fwd: sizes leave no room for a key/value tile in shared memory");
     int64_t cap = 8192;                                      // 32 KB per tile is plenty
@@ -1038,15 +728,11 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
   NM_REQUIRE(smem_bytes <= (size_t)DS_MAX_DYN_SMEM, NM_E_UNSUPPORTED,
              "nm_attn_decoder_step_fwd: needs %zu bytes of shared memory", smem_bytes);
 
-  auto kern = p.R == DS_R_MAX ? attn_decoder_step_kernel<4, false, DS_R_MAX>
-                              : (p.wtma ? attn_decoder_step_kernel<4, true, DS_R>
-                                        : (vec ? attn_decoder_step_kernel<4, false, DS_R>
-                                               : attn_decoder_step_kernel<1, false, DS_R>));
-  static bool attr_done[4] = {false, false, false, false};
-  const int variant = p.R == DS_R_MAX ? 3 : (p.wtma ? 2 : (vec ? 1 : 0));
-  if (!attr_done[variant]) {
+  auto kern = vec ? attn_decoder_step_kernel<4> : attn_decoder_step_kernel<1>;
+  static bool attr_done[2] = {false, false};
+  if (!attr_done[vec]) {
     NM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, DS_MAX_DYN_SMEM));
-    attr_done[variant] = true;
+    attr_done[vec] = true;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(clusters * cl));

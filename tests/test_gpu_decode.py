@@ -48,8 +48,6 @@ def _step_reference(p, symbols, h_prev, parent, group):
     return hn, ctx, w, out
 
 
-@pytest.mark.parametrize("staging", [0, 1, 16])   # weights: 16-byte loads from L2 | 2-D TMA tiles through shared memory
-                                                  # | (16) 16-byte loads with 16 hypotheses per cluster
 @pytest.mark.parametrize("cluster", ["", "1", "2", "4", "8"])
 @pytest.mark.parametrize("dims", [
     # rows, group, E, H, A, C, Tx, O, maxout, masked
@@ -58,7 +56,7 @@ def _step_reference(p, symbols, h_prev, parent, group):
     (24, 3, 32, 40, 64, 64, 50, 32, True, False),      # beam rows sharing an encoder row, no mask
     (64, 8, 300, 300, 600, 600, 50, 300, False, True),  # en-de dims, beam 8
 ])
-def test_step_kernel_against_fp64(monkeypatch, dims, cluster, staging):
+def test_step_kernel_against_fp64(monkeypatch, dims, cluster):
     from neuralmonkey_b200 import lib
     rows, group, e, h, a, c, tx, o, maxout, masked = dims
     monkeypatch.setenv("NMB200_DECSTEP_CLUSTER", cluster)
@@ -88,19 +86,13 @@ def test_step_kernel_against_fp64(monkeypatch, dims, cluster, staging):
     x_out = torch.empty(rows, e, device="cuda")
     sym_d, hp_d = symbols.cuda(), h_prev.cuda()
     par_d = parent.cuda() if parent is not None else None
-    lib.call("nm_attn_decoder_step_set_staging", 0 if staging == 16 else staging)
-    lib.call("nm_attn_decoder_step_set_rows", 16 if staging == 16 else 8)
-    try:
-        lib.call("nm_attn_decoder_step_fwd", lib.ptr(sym_d), lib.ptr(dv["table"]), None, lib.ptr(hp_d), lib.ptr(par_d),
-                 lib.ptr(dv["wg"]), lib.ptr(dv["bg"]), lib.ptr(dv["wc"]), lib.ptr(dv["bc"]), lib.ptr(dv["wq"]),
-                 lib.ptr(dv["bq"]), lib.ptr(dv["v"]), lib.ptr(dv["ab"]), lib.ptr(dv["keys"]), lib.ptr(dv["values"]),
-                 lib.ptr(dv["mask"]), lib.ptr(dv["wo"]), lib.ptr(dv["bo"]), lib.ptr(x_out), lib.ptr(out_h),
-                 lib.ptr(out_ctx), lib.ptr(out_w), lib.ptr(out), rows, group, e, h, a, c, tx, o, 1, int(maxout),
-                 lib.stream())
-        torch.cuda.synchronize()
-    finally:
-        lib.call("nm_attn_decoder_step_set_staging", -1)
-        lib.call("nm_attn_decoder_step_set_rows", -1)
+    lib.call("nm_attn_decoder_step_fwd", lib.ptr(sym_d), lib.ptr(dv["table"]), None, lib.ptr(hp_d), lib.ptr(par_d),
+             lib.ptr(dv["wg"]), lib.ptr(dv["bg"]), lib.ptr(dv["wc"]), lib.ptr(dv["bc"]), lib.ptr(dv["wq"]),
+             lib.ptr(dv["bq"]), lib.ptr(dv["v"]), lib.ptr(dv["ab"]), lib.ptr(dv["keys"]), lib.ptr(dv["values"]),
+             lib.ptr(dv["mask"]), lib.ptr(dv["wo"]), lib.ptr(dv["bo"]), lib.ptr(x_out), lib.ptr(out_h),
+             lib.ptr(out_ctx), lib.ptr(out_w), lib.ptr(out), rows, group, e, h, a, c, tx, o, 1, int(maxout),
+             lib.stream())
+    torch.cuda.synchronize()
     assert torch.equal(x_out.cpu(), p["table"][symbols])
     tol = 3e-5
     assert max_abs(out_h, want[0]) < tol
