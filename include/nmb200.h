@@ -494,6 +494,35 @@ int nm_beam_step_logits(const float* logits, const float* lse, const float* logp
 int nm_beam_backtrack(const int64_t* first_symbols, const int64_t* words, const int32_t* parents,
                       int64_t* token_ids, int64_t B, int64_t k, int64_t steps, void* stream);
 
+/* ---- K16: CTC loss and greedy CTC decoding ---------------------------------------------------------
+ * Replace tf.nn.ctc_loss(ignore_longer_outputs_than_inputs=True, ctc_merge_repeated=merge_repeated) and
+ * tf.nn.ctc_greedy_decoder of decoders/ctc_decoder.py:73-112 (TF 1.12 semantics; preprocess_collapse_repeated
+ * is the caller's job).  logits [B,T,C] batch-major, the blank is class C-1; frames [B] i32: frames
+ * t >= frames[b] are ignored; labels [B,Lmax] i64, row b holding label_lengths[b] (i32) labels in [0, C-1).
+ * nm_ctc_loss_fwd: loss[b] = -log p(labels_b | logits_b), summed over the alignments of the extended label
+ *   (blank, l1, blank, ..., blank) in log space.  merge_repeated != 0 (standard CTC): a state may repeat and
+ *   the skip over a blank needs two different labels; 0: labels do not repeat, every label may be skipped to.
+ *   A sentence whose labels need more frames than it has (L, plus one per pair of equal neighbours with
+ *   merging), or that has no frames, gets loss 0; a label outside [0, C-1) or a length outside [0, Lmax]
+ *   gives NaN.  Both get a zero gradient.
+ * nm_ctc_loss_bwd: dlogits [B,T,C] = grad_loss[b] * (softmax - sum of the occupancies of the states of class k),
+ *   dense, zeros on ignored frames; reads what the forward call left in the workspace and is deterministic.
+ * workspace: at least B*T*(5*Lmax+4) + B*(Lmax+4) 4-byte words (8-byte aligned), passed to both calls;
+ *   workspace_words is its size.  Lmax <= NM_CTC_MAX_LABEL, otherwise NM_E_UNSUPPORTED.
+ * nm_ctc_greedy_decode: per frame the first index of the row maximum; blanks dropped, and with
+ *   merge_repeated a symbol equal to the previous frame's maximum; ids [B,T] i64 padded with 2 (</s>),
+ *   lengths [B] i32 = number of symbols kept. */
+#define NM_CTC_MAX_LABEL 1023
+int nm_ctc_loss_fwd(const float* logits, const int32_t* frames, const int64_t* labels,
+                    const int32_t* label_lengths, int merge_repeated, float* loss, void* workspace,
+                    int64_t workspace_words, int64_t B, int64_t T, int64_t C, int64_t Lmax, void* stream);
+int nm_ctc_loss_bwd(const float* logits, const int32_t* frames, const int64_t* labels,
+                    const int32_t* label_lengths, int merge_repeated, const float* grad_loss, float* dlogits,
+                    void* workspace, int64_t workspace_words, int64_t B, int64_t T, int64_t C, int64_t Lmax,
+                    void* stream);
+int nm_ctc_greedy_decode(const float* logits, const int32_t* frames, int merge_repeated, int64_t* ids,
+                         int32_t* lengths, int64_t B, int64_t T, int64_t C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1140,6 +1140,72 @@ def beam_gather(x: torch.Tensor, beam_ids: torch.Tensor, bsz: int, k: int) -> to
 
 
 # ---------------------------------------------------------------------------
+# K16 CTC loss and greedy CTC decoding
+# ---------------------------------------------------------------------------
+def _ctc_workspace_words(bsz: int, t: int, lmax: int) -> int:
+    return bsz * t * (5 * lmax + 4) + bsz * (lmax + 4)      # the size nm_ctc_loss_fwd documents
+
+
+class _CTCLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, frames, labels, label_lengths, merge_repeated):
+        bsz, t, c = logits.shape
+        lmax = labels.shape[1]
+        words = _ctc_workspace_words(bsz, t, lmax)
+        ws = torch.empty(words, device=logits.device, dtype=torch.float32)
+        loss = torch.empty(bsz, device=logits.device, dtype=torch.float32)
+        call("nm_ctc_loss_fwd", ptr(logits), ptr(frames), ptr(labels), ptr(label_lengths), int(merge_repeated),
+             ptr(loss), ptr(ws), words, bsz, t, c, lmax, lib.stream())
+        ctx.save_for_backward(logits, frames, labels, label_lengths, ws)
+        ctx.merge = int(merge_repeated)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        logits, frames, labels, label_lengths, ws = ctx.saved_tensors
+        bsz, t, c = logits.shape
+        dloss = _f32(dloss).contiguous()
+        dlogits = torch.empty_like(logits)
+        call("nm_ctc_loss_bwd", ptr(logits), ptr(frames), ptr(labels), ptr(label_lengths), ctx.merge, ptr(dloss),
+             ptr(dlogits), ptr(ws), ws.numel(), bsz, t, c, labels.shape[1], lib.stream())
+        return dlogits, None, None, None, None
+
+
+def _ctc_inputs(logits: torch.Tensor, frames: torch.Tensor):
+    if logits.dim() != 3:
+        raise ValueError("CTC logits must be [batch, time, classes], got {}".format(tuple(logits.shape)))
+    if frames.dtype != torch.int32 or frames.shape != (logits.shape[0],):
+        raise ValueError("CTC frames must be int32 [batch]")
+    return _f32(logits).contiguous(), frames.contiguous()
+
+
+def ctc_loss(logits: torch.Tensor, frames: torch.Tensor, labels: torch.Tensor, label_lengths: torch.Tensor,
+             merge_repeated: bool) -> torch.Tensor:
+    """Per-sentence -log p(labels | logits) of tf.nn.ctc_loss(ignore_longer_outputs_than_inputs=True,
+    ctc_merge_repeated=merge_repeated) (decoders/ctc_decoder.py:96-104).  logits [B, T, C] (blank = C-1),
+    frames [B] int32, labels [B, Lmax] int64 (the first label_lengths[b] entries of row b; int32 lengths).
+    Differentiable in the logits: the backward pass returns the dense dlogits."""
+    logits, frames = _ctc_inputs(logits, frames)
+    if labels.dtype != torch.int64 or labels.dim() != 2 or labels.shape[0] != logits.shape[0]:
+        raise ValueError("CTC labels must be int64 [batch, max label length]")
+    if label_lengths.dtype != torch.int32 or label_lengths.shape != (logits.shape[0],):
+        raise ValueError("CTC label lengths must be int32 [batch]")
+    return _CTCLoss.apply(logits, frames, labels.contiguous(), label_lengths.contiguous(), bool(merge_repeated))
+
+
+def ctc_greedy_decode(logits: torch.Tensor, frames: torch.Tensor, merge_repeated: bool):
+    """tf.nn.ctc_greedy_decoder (decoders/ctc_decoder.py:77-80) over batch-major logits [B, T, C]: returns
+    (ids [B, T] int64 padded with </s>, lengths [B] int32)."""
+    logits, frames = _ctc_inputs(logits.detach(), frames)
+    bsz, t, c = logits.shape
+    ids = torch.empty(bsz, t, device=logits.device, dtype=torch.int64)
+    lengths = torch.empty(bsz, device=logits.device, dtype=torch.int32)
+    call("nm_ctc_greedy_decode", ptr(logits), ptr(frames), int(merge_repeated), ptr(ids), ptr(lengths), bsz, t, c,
+         lib.stream())
+    return ids, lengths
+
+
+# ---------------------------------------------------------------------------
 # K12 frozen VGG stack primitives (forward only)
 # ---------------------------------------------------------------------------
 def conv3x3_bias_relu(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:

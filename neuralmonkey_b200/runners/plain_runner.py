@@ -1,12 +1,14 @@
 """PlainRunner (reference: neuralmonkey/runners/plain_runner.py): decodes `decoder.decoded` - the argmax
 over logits[:, :, 1:] + 1 of the greedy loop, i.e. <pad> can never be produced - instead of the runner-side
 argmax of GreedyRunner; a single session only."""
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Union
 
 from neuralmonkey_b200.decoders.autoregressive import AutoregressiveDecoder
+from neuralmonkey_b200.decoders.ctc_decoder import CTCDecoder
 from neuralmonkey_b200.runners.base_runner import BaseRunner
 from neuralmonkey_b200.typecheck import check_argument_types
 
+SupportedDecoder = Union[AutoregressiveDecoder, CTCDecoder]
 Postprocessor = Optional[Callable[[List[List[str]]], List[List[str]]]]
 
 
@@ -26,7 +28,7 @@ class PlainRunner(BaseRunner):
         def execute_sessions(self, activate, num_sessions: int) -> None:
             raise ValueError("PlainRunner needs exactly 1 execution result, got {}".format(num_sessions))
 
-    def __init__(self, output_series: str, decoder: AutoregressiveDecoder,
+    def __init__(self, output_series: str, decoder: SupportedDecoder,
                  postprocess: Postprocessor = None) -> None:
         check_argument_types()
         BaseRunner.__init__(self, output_series, decoder)

@@ -59,6 +59,8 @@ class CostObjective(Objective):
     @property
     def loss_sum_and_count(self):
         dec = self.decoder
+        if hasattr(type(dec), "loss_sum_and_count"):      # a decoder whose cost is not a token mean says how it splits
+            return dec.loss_sum_and_count
         if hasattr(type(dec), "train_xent_sum") and hasattr(type(dec), "_train_mask_bm"):
             return dec.train_xent_sum, dec._train_mask_bm.sum()
         return None
