@@ -161,8 +161,8 @@ int nm_gru_resident_clusters(int backward);
 /* Recurrence engine of nm_gru_seq_fwd/bwd: 0 (default) or 1; on sm_90a both run the persistent cluster
  * kernels in exact fp32 (the mode is recorded for callers that set it). */
 int nm_gru_set_mode(int mode);
-/* Diagnostic: 8 int64 device counters receiving the cycles CTA 0 of the forward cluster
- * kernel spends per section (phase 1: load, dot, gates, barrier; phase 2: same). NULL = off. */
+/* Diagnostic: 8 int64 device counters receiving the cycles thread 0 of CTA 0 of the forward and
+ * backward cluster kernels spends per section of a step (see tools/gru_probe.py). NULL = off. */
 int nm_gru_debug_profile(void* counters);
 /* Inputs: dstates [B,T,H] (may be NULL), dfinal [B,H] (may be NULL).
  * Outputs: dxproj [B,T,3H] (pre-activation grads = grads of xproj), dh0 [B,H]
@@ -176,11 +176,10 @@ int nm_gru_seq_bwd(const float* Wgh, const float* Wch, const int32_t* lengths,
                    const float* dfinal, float* dxproj, float* dh0, float* work,
                    int64_t B, int64_t T, int64_t H, int sm_budget, void* stream);
 
-/* Both directions of a bidirectional layer (tf.nn.bidirectional_dynamic_rnn, encoders/recurrent.py:82-95)
- * in ONE launch of the tensor-core engine: the clusters of sequence a and of sequence b are co-resident
- * (each direction alone fills only half of the chip for the length of the sentence).  Same arguments as
- * nm_gru_seq_fwd / nm_gru_seq_bwd per sequence, without h0 / drop_mask / raw_states (encoder layers have
- * none); `lengths` is shared.  Falls back to two launches where the tensor-core engine does not apply. */
+/* Both directions of a bidirectional layer (tf.nn.bidirectional_dynamic_rnn, encoders/recurrent.py:82-95):
+ * sequence a, then sequence b, each as one nm_gru_seq_fwd / nm_gru_seq_bwd call on the whole GPU.  Same
+ * arguments as nm_gru_seq_fwd / nm_gru_seq_bwd per sequence, without h0 / drop_mask / raw_states (encoder
+ * layers have none); `lengths` is shared. */
 int nm_gru_seq_fwd_pair(const float* xproj_a, const float* Wgh_a, const float* Wch_a, int reverse_a,
                         float* states_a, float* final_a, float* gates_a, float* hprev_a, float* rh_a,
                         const float* xproj_b, const float* Wgh_b, const float* Wch_b, int reverse_b,

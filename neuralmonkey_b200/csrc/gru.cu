@@ -145,7 +145,7 @@ bool cluster_path_ok(int64_t H) {
 int g_gru_mode = 0;   // nm_gru_set_mode(): recorded; every mode runs the cluster engine on sm_90a
 
 struct ClusterPlan {
-  int Bc, nclusters, ch;
+  int Bc, nclusters, sl;
   size_t smem;
 };
 
@@ -166,7 +166,7 @@ int max_active_clusters(Kern kern, size_t smem) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess ||
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GC_SMEM_CAP) != cudaSuccess ||
       cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n < 1) {
     cudaGetLastError();
     n = sm_count() / GC_CLUSTER / 2;
@@ -174,32 +174,31 @@ int max_active_clusters(Kern kern, size_t smem) {
   return n;
 }
 
+// One CTA per SM whatever the shared-memory footprint (the register file is the limit), so the
+// widest instance at a typical footprint stands for all of them.
 int resident_clusters(bool backward) {
   static int cached[2] = {0, 0};
   if (cached[backward] == 0)
-    cached[backward] = backward ? max_active_clusters(gru_seq_bwd_cluster_kernel<3>, 64 * 1024)
-                                : max_active_clusters(gru_seq_fwd_cluster_kernel<3>, 64 * 1024);
+    cached[backward] = backward ? max_active_clusters(gru_seq_bwd_cluster_kernel<GC_MAX_SL>, 128 * 1024)
+                                : max_active_clusters(gru_seq_fwd_cluster_kernel<GC_MAX_SL>, 128 * 1024);
   return cached[backward];
 }
 
 ClusterPlan plan_clusters(int64_t B, int64_t H, int sm_budget, bool backward) {
-  const int SL32 = (int)((H + GC_SLICES - 1) / GC_SLICES);
   ClusterPlan p;
-  p.ch = (SL32 + 3) / 4;  // 1, 2 or 3 for H <= 320
-  const int ROW = GC_SLICES * 4 * (p.ch | 1);
+  p.sl = (int)((H + GC_SLICES - 1) / GC_SLICES);  // 1..10 for H <= 320
   int max_clusters = resident_clusters(backward);
   if (sm_budget > 0 && sm_budget / GC_CLUSTER < max_clusters) max_clusters = sm_budget / GC_CLUSTER;
   if (max_clusters < 1) max_clusters = 1;
   int Bc = (int)((B + max_clusters - 1) / max_clusters);
   Bc = (Bc + 3) / 4 * 4;
-  const size_t per_row = backward ? (size_t)(2 * ROW + 3 * GC_MAX_UNITS) * 4
-                                  : (size_t)(ROW + 7 * GC_MAX_UNITS) * 4;
-  const int cap = (int)((200 * 1024) / per_row) / 4 * 4;
+  const size_t per_row = (size_t)(backward ? gc_bwd_row_floats(p.sl) : gc_fwd_row_floats(p.sl)) * 4;
+  const int cap = (int)((GC_SMEM_CAP - GC_BAR_BYTES) / per_row) / 4 * 4;
   if (Bc > cap) Bc = cap;
   if (Bc < 4) Bc = 4;
   p.Bc = Bc;
   p.nclusters = (int)((B + Bc - 1) / Bc);
-  p.smem = per_row * Bc;
+  p.smem = GC_BAR_BYTES + per_row * Bc;
   return p;
 }
 
@@ -223,11 +222,18 @@ int launch_cluster(Kern kern, const Args& args, const ClusterPlan& p, cudaStream
   return NM_OK;
 }
 
-#define NM_GC_DISPATCH(KERN, args, plan, s, name)                   \
-  switch ((plan).ch) {                                              \
-    case 1: return launch_cluster(KERN<1>, args, plan, s, name);    \
-    case 2: return launch_cluster(KERN<2>, args, plan, s, name);    \
-    default: return launch_cluster(KERN<3>, args, plan, s, name);   \
+#define NM_GC_DISPATCH(KERN, args, plan, s, name)                  \
+  switch ((plan).sl) {                                             \
+    case 1: return launch_cluster(KERN<1>, args, plan, s, name);   \
+    case 2: return launch_cluster(KERN<2>, args, plan, s, name);   \
+    case 3: return launch_cluster(KERN<3>, args, plan, s, name);   \
+    case 4: return launch_cluster(KERN<4>, args, plan, s, name);   \
+    case 5: return launch_cluster(KERN<5>, args, plan, s, name);   \
+    case 6: return launch_cluster(KERN<6>, args, plan, s, name);   \
+    case 7: return launch_cluster(KERN<7>, args, plan, s, name);   \
+    case 8: return launch_cluster(KERN<8>, args, plan, s, name);   \
+    case 9: return launch_cluster(KERN<9>, args, plan, s, name);   \
+    default: return launch_cluster(KERN<10>, args, plan, s, name); \
   }
 
 }  // namespace
@@ -243,8 +249,9 @@ int nm_gru_set_mode(int mode) {
 }
 
 static long long* g_gru_prof = nullptr;
-/* Diagnostic: device buffer of 8 int64 cycle counters filled by CTA 0 of the next forward
- * cluster launches (load, dot, gate, barrier for each of the two phases); NULL disables. */
+/* Diagnostic: device buffer of 8 int64 cycle counters accumulated by thread 0 of CTA 0 of the next
+ * cluster launches, forward and backward alike (the slots are listed in tools/gru_probe.py); NULL
+ * disables. */
 int nm_gru_debug_profile(void* counters) {
   g_gru_prof = reinterpret_cast<long long*>(counters);
   return NM_OK;
@@ -301,7 +308,7 @@ int nm_gru_seq_bwd(const float* Wgh, const float* Wch, const int32_t* lengths,
   cudaStream_t s = (cudaStream_t)stream;
   if (cluster_path_ok(H)) {
     GcBwdArgs a{Wgh, Wch, lengths, drop_mask, gates, hprev, dstates, draw, dfinal, dxproj, dh0,
-                (int)B, (int)T, (int)H, 0, reverse};
+                (int)B, (int)T, (int)H, 0, reverse, g_gru_prof};
     const ClusterPlan p = plan_clusters(B, H, sm_budget, true);
     a.Bc = p.Bc;
     NM_GC_DISPATCH(gru_seq_bwd_cluster_kernel, a, p, s, "nm_gru_seq_bwd(cluster)");

@@ -1,20 +1,26 @@
 // Persistent GRU sequence kernels for thread-block clusters (sm_90a).
 //
 // One launch runs the whole time loop.  A cluster of 8 CTAs owns a slice of the batch
-// (Bc sentences); inside it, CTA r owns hidden units [r*UW, (r+1)*UW), UW = ceil(H/8).
+// (Bc sentences); inside it, CTA r owns hidden units [r*H/8, (r+1)*H/8): at least one each
+// (H >= 8), at most ceil(H/8) <= 40, so every CTA sends its share of every exchanged vector.
 // The recurrent weights never leave the SM: a warp owns 4 hidden units, and each of its
 // 32 lanes keeps, in REGISTERS, the three weight vectors of those 4 units restricted to
-// ONE of 32 reduction slices (3 * 4 * 4*CH floats per thread).  The inner product then
-// streams only the state vector from shared memory - one conflict-free 16-byte load
-// feeds 32 (gates) or 16 (candidate) FMAs - and is FMA-issue bound.  The 32 partial sums
-// of a (row, unit) pair are combined with five shuffle steps.
+// ONE of 32 reduction slices of SL = ceil(H/32) elements (3 * 4 * SL floats per thread, 120
+// at H = 300).  The inner product streams only the state vector from shared memory in 16-,
+// 8- and 4-byte pieces of exactly SL elements and is FMA-issue bound.  The 32 partial sums
+// of a (row, unit) pair are combined with a reduce-scatter over shuffles.
 //
 // The two matmuls of a TF GRUCell step are dependent (the candidate needs r*h for ALL
-// units), so a step has two phases separated by hardware cluster barriers; the vectors
-// exchanged between the phases (h, r*h; backward: dz_c, dz_u, dz_r) are exactly the
-// tensors the backward pass / the weight-gradient GEMMs need in HBM anyway, so the
-// exchange costs only an L2 read of Bc*H floats per CTA per phase.  Element-wise gate
-// math runs as a separate pass with threads along the hidden axis (coalesced HBM access).
+// units).  The lanes that end up holding a reduced sum apply the gate math themselves and
+// write the result - r*h or h' forward, dz_c / dz_u / dz_r backward - straight into the
+// vector buffer of every CTA of the cluster with st.async, whose bytes are counted on a
+// transaction mbarrier of the receiving CTA.  A CTA starts a phase as soon as its barrier has
+// counted the whole Bc x H vector: no cluster-wide barrier and no L2 round trip in the loop.
+// Write-after-read hazards are ordered by the dataflow itself: a peer can only send the next
+// value of a buffer after it has received this CTA's contribution to the phase that follows
+// the last read of that buffer; the buffers for which that is not enough (forward h,
+// backward dz_u) alternate by step parity.  The saved activations (states, gates, hprev, rh,
+// dxproj) go to global memory off the critical path.
 #pragma once
 #include "common.cuh"
 
@@ -28,6 +34,31 @@ constexpr int GC_WARPS = 10;    // -> up to 40 units per CTA (H <= 320); 3 warps
 constexpr int GC_THREADS = GC_WARPS * 32;
 constexpr int GC_MAX_UNITS = GC_WARPS * GC_UPW;
 constexpr int GC_RB = 2;        // batch rows per inner iteration
+constexpr int GC_MAX_SL = 10;   // ceil(320 / 32)
+constexpr int GC_SMEM_CAP = 200 * 1024;  // dynamic shared memory a launch may plan for
+constexpr int GC_BAR_BYTES = 64;  // transaction barriers at the start of dynamic shared memory
+constexpr int GC_XS = 4;        // forward prefetch per (row, unit): xproj r, u, c and the dropout mask
+constexpr int GC_PF = 8;        // backward prefetch per (row, unit): r, u, c, h, dstates, drop mask, draw
+
+// Geometry: SLP = slice pitch in the smem vector buffer, an odd number of 16-byte chunks so
+// the 32 lanes of a 16-byte load fall into 4 conflict-free quarter-warp wavefronts;
+// ROW = 32*SLP floats per batch row.  Only the first SL floats of a slice are ever read.
+__host__ __device__ constexpr int gc_row(int SL) { return GC_SLICES * 4 * (((SL + 3) / 4) | 1); }
+// floats of dynamic shared memory per batch row, after the barrier block
+__host__ __device__ constexpr int gc_fwd_row_floats(int SL) {
+  return 3 * gc_row(SL) + GC_MAX_UNITS * (1 + 2 * GC_XS) + 1;
+}
+__host__ __device__ constexpr int gc_bwd_row_floats(int SL) {
+  return 4 * gc_row(SL) + GC_MAX_UNITS * (1 + 2 * GC_PF) + 1;
+}
+
+template <int SL>
+struct GcGeom {
+  static constexpr int SLP = 4 * (((SL + 3) / 4) | 1);
+  static constexpr int ROW = GC_SLICES * SLP;
+  // offset of hidden unit j inside a row of the sliced layout
+  static __device__ __forceinline__ int pos(int j) { return (j / SL) * SLP + (j % SL); }
+};
 
 __device__ __forceinline__ void cluster_barrier() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::
@@ -38,158 +69,147 @@ __device__ __forceinline__ uint32_t cluster_rank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ float reduce32(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
+
+// --- transaction barriers and distributed shared memory --------------------------------
+__device__ __forceinline__ uint32_t gc_smem_u32(const void* p) {
+  return (uint32_t)__cvta_generic_to_shared(p);
 }
+__device__ __forceinline__ void gc_mbar_init(uint32_t bar) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+// One local arrival that also expects `bytes` of st.async data for the barrier's current phase.
+// Data may arrive before it (the transaction count goes negative); the phase completes when both
+// the arrival and all the bytes are in.
+__device__ __forceinline__ void gc_mbar_arm(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void gc_mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+  } while (!done);
+}
+// Store v at shared-memory address `addr` of CTA `dst` of the cluster (the same layout in every
+// CTA); the 4 bytes are counted on that CTA's barrier at `bar`.
+__device__ __forceinline__ void gc_send(uint32_t addr, uint32_t bar, uint32_t dst, float v) {
+  uint32_t ra, rb;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(addr), "r"(dst));
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(bar), "r"(dst));
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra),
+               "r"(__float_as_uint(v)), "r"(rb)
+               : "memory");
+}
+
+__device__ __forceinline__ void cp_async4(float* smem_dst, const float* gmem_src) {
+  const uint32_t d = gc_smem_u32(smem_dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // Sum N values across the 32 lanes with N-1+log2(32/N)... shuffles instead of 5N: each
 // butterfly level halves the number of live values (lanes whose bit `o` is set keep the
 // upper half and send the lower, and vice versa).  On return v[0] of lane L is the full
 // sum of the value with index (L >> (5 - log2 N)) & (N-1); lanes differing only in the
 // low bits hold copies.
-template <int N>
-__device__ __forceinline__ void gc_reduce_scatter(float (&v)[N], int lane) {
-  int o = 16;
-#pragma unroll
-  for (int n = N; n > 1; n >>= 1) {
-    const bool upper = (lane & o) != 0;
+// One butterfly level per instantiation, O = shuffle distance (a loop over the levels is not
+// always unrolled, and a rolled loop indexes v at run time, which puts v in local memory).
+template <int N, int O>
+__device__ __forceinline__ void gc_reduce_level(float (&v)[N], int lane) {
+  constexpr int n = N * O / 16;  // values still live at this level
+  if constexpr (n > 1) {
+    const bool upper = (lane & O) != 0;
 #pragma unroll
     for (int i = 0; i < n / 2; ++i) {
       const float keep = upper ? v[i + n / 2] : v[i];
       const float send = upper ? v[i] : v[i + n / 2];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);
     }
-    o >>= 1;
+  } else {
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], O);
   }
-  for (; o > 0; o >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
+  if constexpr (O > 1) gc_reduce_level<N, O / 2>(v, lane);
+}
+template <int N>
+__device__ __forceinline__ void gc_reduce_scatter(float (&v)[N], int lane) {
+  gc_reduce_level<N, 16>(v, lane);
 }
 
-// Geometry: SL32 = ceil(H/32) reduction-slice length (<= 4*CH); SLP = slice pitch in the
-// smem vector buffer: an odd number of 16-byte chunks so the 32 lanes of a 16-byte load
-// fall into 4 conflict-free quarter-warp wavefronts; ROW = 32*SLP floats per batch row.
-template <int CH>
-struct GcGeom {
-  static constexpr int SLP = 4 * (CH | 1);
-  static constexpr int ROW = GC_SLICES * SLP;
-};
-
-// Stage H contiguous floats per row into the sliced layout.  Thread t owns columns
-// t, t+GC_THREADS, ... (coalesced along the hidden axis); rows >= nrows are zero-filled.
-// Per-thread constants of the loader: thread t owns the 16-byte column group k4 = t % QL
-// (QL = ceil(H/4) rounded so that GC_THREADS % QL rows are handled in parallel) and the
-// row lane t / QL; the four smem offsets of its columns are computed once per kernel.
-struct GcLoader {
-  int k, row_lane, row_lanes, off[4];
-  bool active, vec4;
-};
-
-template <int CH>
-__device__ __forceinline__ GcLoader gc_make_loader(int H, int SL32) {
-  GcLoader L;
-  const int q = (H + 3) >> 2;
-  L.row_lanes = GC_THREADS / q > 0 ? GC_THREADS / q : 1;
-  L.row_lane = threadIdx.x / q;
-  L.k = (threadIdx.x % q) * 4;
-  L.active = (threadIdx.x < q * L.row_lanes);
-  L.vec4 = (H & 3) == 0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int k = L.k + i;
-    L.off[i] = (k < H) ? (k / SL32) * GcGeom<CH>::SLP + (k % SL32) : -1;
-  }
-  return L;
-}
-
-template <int CH>
-__device__ __forceinline__ void gc_load_vec(float* __restrict__ vec, const float* __restrict__ src,
-                                            int64_t pitch, int nrows, int Bc, const GcLoader& L) {
-  constexpr int NB = 8;  // loads in flight per thread: issue all, then store (in-order issue
-                         // would otherwise serialise one L2 round trip per load)
-  constexpr int ROW = GcGeom<CH>::ROW;
-  if (!L.active) return;
-  const bool vec4 = L.vec4 && ((pitch & 3) == 0) && ((reinterpret_cast<uintptr_t>(src) & 15) == 0);
-  for (int b0 = L.row_lane; b0 < Bc; b0 += NB * L.row_lanes) {
-    float4 v[NB];
-#pragma unroll
-    for (int i = 0; i < NB; ++i) {
-      const int b = b0 + i * L.row_lanes;
-      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (b < nrows) {
-        const float* p = src + (int64_t)b * pitch + L.k;
-        if (vec4) {
-          v[i] = __ldcg(reinterpret_cast<const float4*>(p));
-        } else {
-          if (L.off[0] >= 0) v[i].x = __ldcg(p);
-          if (L.off[1] >= 0) v[i].y = __ldcg(p + 1);
-          if (L.off[2] >= 0) v[i].z = __ldcg(p + 2);
-          if (L.off[3] >= 0) v[i].w = __ldcg(p + 3);
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < NB; ++i) {
-      const int b = b0 + i * L.row_lanes;
-      if (b < Bc) {
-        float* row = vec + b * ROW;
-        if (L.off[0] >= 0) row[L.off[0]] = v[i].x;
-        if (L.off[1] >= 0) row[L.off[1]] = v[i].y;
-        if (L.off[2] >= 0) row[L.off[2]] = v[i].z;
-        if (L.off[3] >= 0) row[L.off[3]] = v[i].w;
-      }
-    }
-  }
-}
-
-__device__ __forceinline__ void cp_async4(float* smem_dst, const float* gmem_src) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit_wait_all() {
-  asm volatile("cp.async.commit_group;\n\tcp.async.wait_all;" ::: "memory");
-}
-
-// acc[r][u] = partial (this lane's slice) of sum_k vec[row0+r][k] * w[u][k]
-template <int CH>
+// acc[r][u] = partial (this lane's slice) of sum_k vec[row0+r][k] * w[u][k], over exactly the SL
+// elements of the slice (16-byte pieces, then an 8- and a 4-byte one as SL requires)
+template <int SL>
 __device__ __forceinline__ void gc_dot(const float* __restrict__ vec, int row0, int lane,
-                                       const float (&w)[GC_UPW][4 * CH], float (&acc)[GC_RB][GC_UPW]) {
+                                       const float (&w)[GC_UPW][SL], float (&acc)[GC_RB][GC_UPW]) {
 #pragma unroll
   for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
     for (int u = 0; u < GC_UPW; ++u) acc[r][u] = 0.f;
-  const float* base = vec + row0 * GcGeom<CH>::ROW + lane * GcGeom<CH>::SLP;
+  const float* base = vec + row0 * GcGeom<SL>::ROW + lane * GcGeom<SL>::SLP;
 #pragma unroll
-  for (int c = 0; c < CH; ++c) {
+  for (int c = 0; c < SL; c += 4) {
+    const int n = SL - c < 4 ? SL - c : 4;
 #pragma unroll
     for (int r = 0; r < GC_RB; ++r) {
-      const float4 v = *reinterpret_cast<const float4*>(base + r * GcGeom<CH>::ROW + 4 * c);
-#pragma unroll
-      for (int u = 0; u < GC_UPW; ++u) {
-        acc[r][u] = fmaf(v.x, w[u][4 * c], acc[r][u]);
-        acc[r][u] = fmaf(v.y, w[u][4 * c + 1], acc[r][u]);
-        acc[r][u] = fmaf(v.z, w[u][4 * c + 2], acc[r][u]);
-        acc[r][u] = fmaf(v.w, w[u][4 * c + 3], acc[r][u]);
+      const float* p = base + r * GcGeom<SL>::ROW + c;
+      float x[4];
+      if (n == 4) {
+        const float4 q = *reinterpret_cast<const float4*>(p);
+        x[0] = q.x; x[1] = q.y; x[2] = q.z; x[3] = q.w;
+      } else {
+        if (n >= 2) {
+          const float2 q = *reinterpret_cast<const float2*>(p);
+          x[0] = q.x; x[1] = q.y;
+        }
+        if (n == 1) x[0] = p[0];
+        if (n == 3) x[2] = p[2];
       }
+#pragma unroll
+      for (int u = 0; u < GC_UPW; ++u)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (i < n) acc[r][u] = fmaf(x[i], w[u][c + i], acc[r][u]);
     }
   }
 }
 
 // Load this lane's slice of column (or row) vectors of a weight matrix for the warp's 4
-// units: w[u][i] = W[(k0+i)*sk + unit(u)*su] for i < SL32, zero elsewhere.
-template <int CH>
-__device__ __forceinline__ void gc_load_w(float (&w)[GC_UPW][4 * CH], const float* __restrict__ W,
-                                          int64_t sk, int64_t su, int unit0, int nunits_total,
-                                          int unit_limit, int k0, int SL32, int H) {
+// units: w[u][i] = W[(k0+i)*sk + unit(u)*su], zero past H or past the CTA's units.
+template <int SL>
+__device__ __forceinline__ void gc_load_w(float (&w)[GC_UPW][SL], const float* __restrict__ W,
+                                          int64_t sk, int64_t su, int unit0, int unit_limit, int k0, int H) {
 #pragma unroll
   for (int u = 0; u < GC_UPW; ++u)
 #pragma unroll
-    for (int i = 0; i < 4 * CH; ++i) {
+    for (int i = 0; i < SL; ++i) {
       const int unit = unit0 + u, k = k0 + i;
-      const bool ok = (unit < unit_limit) && (unit < nunits_total) && (i < SL32) && (k < H);
+      const bool ok = (unit < unit_limit) && (k < H);
       w[u][i] = ok ? W[(int64_t)k * sk + (int64_t)unit * su] : 0.f;
     }
 }
+
+// Per-phase cycle counters of thread 0 of CTA 0 (diagnostics; see nm_gru_debug_profile).  The
+// running timestamp is a 32-bit clock() (differences are exact across a wrap) and the counters
+// are read from the kernel parameters, so profiling costs two registers in the step loop.
+struct GcProf {
+  bool on;
+  unsigned t0;
+  __device__ __forceinline__ explicit GcProf(const long long* out)
+      : on(out != nullptr && blockIdx.x == 0 && threadIdx.x == 0), t0(on ? (unsigned)clock() : 0u) {}
+  __device__ __forceinline__ void lap(long long* out, int slot) {
+    if (on) {
+      const unsigned t1 = (unsigned)clock();
+      out[slot] += (long long)(t1 - t0);
+      t0 = t1;
+    }
+  }
+};
 
 // ---------------------------------------------------------------------------
 // forward
@@ -211,151 +231,201 @@ struct GcFwdArgs {
   long long* prof;      // optional [8] cycle counters of CTA 0 (diagnostics), or null
 };
 
-template <int CH>
+// Asynchronous copies of step t's xproj (and dropout mask) of the own units into the prefetch slot
+// `dst` ([Bc][GC_MAX_UNITS][GC_XS]); they land while the previous step computes.
+__device__ __forceinline__ void gc_fwd_prefetch(const GcFwdArgs& a, int t, float* dst, int b0, int nrows,
+                                                int ubeg, int UW) {
+  const int H = a.H, T = a.T;
+  for (int idx = threadIdx.x; idx < a.Bc * UW; idx += GC_THREADS) {
+    const int b = idx / UW, ul = idx - b * UW, j = ubeg + ul;
+    if (b < nrows && j < H) {
+      const int64_t row = ((int64_t)(b0 + b) * T + t);
+      const float* xp = a.xproj + row * 3 * H + j;
+      float* xd = dst + (b * GC_MAX_UNITS + ul) * GC_XS;
+      cp_async4(xd, xp);
+      cp_async4(xd + 1, xp + H);
+      cp_async4(xd + 2, xp + 2 * H);
+      if (a.drop_mask) cp_async4(xd + 3, a.drop_mask + row * H + j);
+    }
+  }
+  cp_async_commit();
+}
+
+// Bytes of one exchanged Bc x H vector.  Recomputed from the kernel parameters where it is used, so
+// that it holds no register across the step loop (the SL = 10 instance is at the 168-register cap).
+__device__ __forceinline__ uint32_t gc_phase_bytes(const GcFwdArgs& a) { return (uint32_t)(a.Bc * a.H * 4); }
+
+template <int SL>
 __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFwdArgs a) {
   extern __shared__ __align__(16) float gc_smem[];
-  constexpr int ROW = GcGeom<CH>::ROW;
-  float* vec = gc_smem;                 // [Bc][ROW]
-  float* pre = vec + a.Bc * ROW;        // [Bc][GC_MAX_UNITS][2] pre-activations
-  float* own = pre + a.Bc * GC_MAX_UNITS * 2;  // [Bc][GC_MAX_UNITS][2]: (h, u) of own units
-  float* xs = own + a.Bc * GC_MAX_UNITS * 2;   // [Bc][GC_MAX_UNITS][3]: this step's xproj
+  constexpr int ROW = GcGeom<SL>::ROW;
   const int H = a.H, T = a.T, Bc = a.Bc;
-  const int UW = (H + GC_CLUSTER - 1) / GC_CLUSTER;   // units per CTA
-  const int SL32 = (H + GC_SLICES - 1) / GC_SLICES;   // reduction slice length
+  float* hbuf = gc_smem + GC_BAR_BYTES / 4;          // [2][Bc][ROW]: h by step parity
+  float* rhbuf = hbuf + 2 * Bc * ROW;                // [Bc][ROW]: r*h
+  float* us = rhbuf + Bc * ROW;                      // [Bc][GC_MAX_UNITS]: update gate of own units
+  float* xs = us + Bc * GC_MAX_UNITS;                // [2][Bc][GC_MAX_UNITS][GC_XS] by step parity
+  int* lens = reinterpret_cast<int*>(xs + 2 * Bc * GC_MAX_UNITS * GC_XS);  // [Bc]; 0 for padding rows
+  const uint32_t bar_h = gc_smem_u32(gc_smem), bar_rh = bar_h + 16;      // bar_h + 8*parity
+
   const int rank = (int)cluster_rank();
+  const int ubeg = rank * H / GC_CLUSTER;             // first hidden unit of this CTA
+  const int unit_limit = (rank + 1) * H / GC_CLUSTER;
+  const int UW = unit_limit - ubeg;                   // units of this CTA
   const int b0 = (blockIdx.x / GC_CLUSTER) * Bc;
   const int nrows = min(Bc, a.B - b0);
-  const GcLoader loader = gc_make_loader<CH>(H, SL32);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int unit0_local = warp * GC_UPW;
-  const int unit0 = rank * UW + unit0_local;          // first hidden unit of this warp
-  const int unit_limit = min(H, (rank + 1) * UW);
+  const int unit0 = ubeg + unit0_local;               // first hidden unit of this warp
+  const bool warp_live = unit0 < unit_limit;
 
-  float wr[GC_UPW][4 * CH], wu[GC_UPW][4 * CH], wc[GC_UPW][4 * CH];
-  gc_load_w<CH>(wr, a.Wgh, 2 * H, 1, unit0, H, unit_limit, lane * SL32, SL32, H);
-  gc_load_w<CH>(wu, a.Wgh + H, 2 * H, 1, unit0, H, unit_limit, lane * SL32, SL32, H);
-  gc_load_w<CH>(wc, a.Wch, H, 1, unit0, H, unit_limit, lane * SL32, SL32, H);
+  float wr[GC_UPW][SL], wu[GC_UPW][SL], wc[GC_UPW][SL];
+  gc_load_w<SL>(wr, a.Wgh, 2 * H, 1, unit0, unit_limit, lane * SL, H);
+  gc_load_w<SL>(wu, a.Wgh + H, 2 * H, 1, unit0, unit_limit, lane * SL, H);
+  gc_load_w<SL>(wc, a.Wch, H, 1, unit0, unit_limit, lane * SL, H);
 
-  // the slice padding of the vector buffer is never written again: it must be 0, not
-  // stale shared memory (NaN * 0-weight would poison the sums)
-  for (int i = threadIdx.x; i < Bc * ROW; i += GC_THREADS) vec[i] = 0.f;
-  // seed the state history slot of the first step with h0 (own units, own rows)
+  // The (row, unit) result this lane holds after each reduce-scatter, fixed for the kernel.
+  // Phase 1: 16 values (gate, row, unit), 2 copies; phase 2: 8 values (row, unit), 4 copies.
+  const int g1 = lane >> 4, r1 = (lane >> 3) & 1, u1 = (lane >> 1) & 3;
+  const int r2 = (lane >> 4) & 1, u2 = (lane >> 2) & 3, copy2 = lane & 3;
+  const int copy1 = ((lane >> 4) << 1) | (lane & 1);  // 4 lanes send each r*h value (see below)
+  const bool ok1 = unit0 + u1 < unit_limit, ok2 = unit0 + u2 < unit_limit;
+  const int j1 = unit0 + u1, j2 = unit0 + u2;
+  const int pos1 = ok1 ? GcGeom<SL>::pos(j1) : 0, pos2 = ok2 ? GcGeom<SL>::pos(j2) : 0;
+
+  if (threadIdx.x == 0) {
+    gc_mbar_init(bar_h);
+    gc_mbar_init(bar_h + 8);
+    gc_mbar_init(bar_rh);
+    gc_mbar_arm(bar_h, gc_phase_bytes(a));
+    gc_mbar_arm(bar_h + 8, gc_phase_bytes(a));
+    gc_mbar_arm(bar_rh, gc_phase_bytes(a));
+  }
+  // The slice padding of the vector buffers is never written: it must be 0, not stale shared
+  // memory; padding rows (and units of the prefetch that are never loaded) stay 0 as well.
+  for (int i = threadIdx.x; i < 3 * Bc * ROW; i += GC_THREADS) hbuf[i] = 0.f;
+  for (int i = threadIdx.x; i < 2 * Bc * GC_MAX_UNITS * GC_XS; i += GC_THREADS) xs[i] = 0.f;
+  for (int b = threadIdx.x; b < Bc; b += GC_THREADS)
+    lens[b] = b < nrows ? (a.lengths ? a.lengths[b0 + b] : T) : 0;
+
+
+  __syncthreads();
+  cluster_barrier();  // every CTA's barriers are initialised and its buffers zeroed before anyone sends
+  // seed: the state history slot of the first step gets h0, and the h0 slice of the own units goes
+  // to h buffer 0 of every CTA
   const int t_first = a.reverse ? T - 1 : 0;
   for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-    const int b = idx / UW, j = rank * UW + (idx - b * UW);
-    if (b < nrows && j < H)
-      a.hprev[((int64_t)(b0 + b) * T + t_first) * H + j] = a.h0 ? a.h0[(int64_t)(b0 + b) * H + j] : 0.f;
+    const int b = idx / UW, j = ubeg + (idx - b * UW);
+    const float hv = (b < nrows && a.h0) ? a.h0[(int64_t)(b0 + b) * H + j] : 0.f;
+    if (b < nrows) a.hprev[((int64_t)(b0 + b) * T + t_first) * H + j] = hv;
+    const uint32_t addr = gc_smem_u32(hbuf + b * ROW + GcGeom<SL>::pos(j));
+    for (int d = 0; d < GC_CLUSTER; ++d) gc_send(addr, bar_h, d, hv);
   }
-  cluster_barrier();
+  gc_fwd_prefetch(a, t_first, xs, b0, nrows, ubeg, UW);
 
+  GcProf prof(a.prof);
   for (int step = 0; step < T; ++step) {
     const int t = a.reverse ? T - 1 - step : step;
     const bool last = (step == T - 1);
     const int t_next = a.reverse ? t - 1 : t + 1;
     const int64_t row0 = (int64_t)b0 * T + t;  // row index of batch row b0 at time t; +b*T per row
+    const int par = step & 1;
+    const float* hb = hbuf + par * Bc * ROW;
+    const float* xc = xs + par * Bc * GC_MAX_UNITS * GC_XS;
 
-    // ---- phase 1: [r,u] = sigmoid(xg + h.Wgh), rh = r*h ----
-    long long tp0 = 0, tp1 = 0;
-    const bool profiling = a.prof != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
-#define GC_PROF(slot) do { if (profiling) { tp1 = clock64(); a.prof[slot] += tp1 - tp0; tp0 = tp1; } } while (0)
-    if (profiling) tp0 = clock64();
-    // issue this step's xproj reads now (cold HBM lines) as asynchronous copies into smem:
-    // they land while the dot products run and cost no registers
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, j = rank * UW + ul;
-      if (b < nrows && j < H) {
-        const float* xp = a.xproj + (row0 + (int64_t)b * T) * 3 * H + j;
-        float* xd = xs + (b * GC_MAX_UNITS + ul) * 3;
-        cp_async4(xd, xp);
-        cp_async4(xd + 1, xp + H);
-        cp_async4(xd + 2, xp + 2 * H);
-      }
-    }
-    gc_load_vec<CH>(vec, a.hprev + row0 * H, (int64_t)T * H, nrows, Bc, loader);
-    __syncthreads();
-    GC_PROF(0);
-    // (no branch around the shuffles: warps past the last unit run on zero weights, which
-    //  keeps every shuffle convergent and free of WARPSYNC.COLLECTIVE wrappers)
-    for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
-      float ar[GC_RB][GC_UPW], au[GC_RB][GC_UPW];
-      gc_dot<CH>(vec, r0, lane, wr, ar);
-      gc_dot<CH>(vec, r0, lane, wu, au);
-      float v[2 * GC_RB * GC_UPW];  // index = gate*8 + row*4 + unit
+    gc_mbar_wait(bar_h + 8 * par, (step >> 1) & 1);
+    if (threadIdx.x == 0 && step + 2 < T) gc_mbar_arm(bar_h + 8 * par, gc_phase_bytes(a));
+    prof.lap(a.prof, 0);
+    cp_async_wait_all();
+    __syncthreads();  // this step's xproj is in; every warp is done with the previous step
+    if (!last) gc_fwd_prefetch(a, t_next, xs + (par ^ 1) * Bc * GC_MAX_UNITS * GC_XS, b0, nrows, ubeg, UW);
+    prof.lap(a.prof, 1);
+
+    // ---- phase 1: [r,u] = sigmoid(xg + h.Wgh), r*h -> every CTA ----
+    // (warps past the last unit skip the loop as a whole, which keeps every shuffle convergent)
+    if (warp_live) {
+      for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
+        float ar[GC_RB][GC_UPW], au[GC_RB][GC_UPW];
+        gc_dot<SL>(hb, r0, lane, wr, ar);
+        gc_dot<SL>(hb, r0, lane, wu, au);
+        float v[2 * GC_RB * GC_UPW];  // index = gate*8 + row*4 + unit
 #pragma unroll
-      for (int r = 0; r < GC_RB; ++r)
+        for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
-        for (int u = 0; u < GC_UPW; ++u) {
-          v[r * GC_UPW + u] = ar[r][u];
-          v[GC_RB * GC_UPW + r * GC_UPW + u] = au[r][u];
+          for (int u = 0; u < GC_UPW; ++u) {
+            v[r * GC_UPW + u] = ar[r][u];
+            v[GC_RB * GC_UPW + r * GC_UPW + u] = au[r][u];
+          }
+        gc_reduce_scatter<2 * GC_RB * GC_UPW>(v, lane);
+        const int b = r0 + r1, ul = unit0_local + u1;
+        const float g = sigmoidf_(v[0] + xc[(b * GC_MAX_UNITS + ul) * GC_XS + g1]);
+        const float rhv = g * hb[b * ROW + pos1];
+        // lanes L and L^16 hold r and u of the same (row, unit): the u lanes help send r*h
+        // (the shuffle runs on every lane: a shuffle skipped by some lanes of its mask never completes)
+        const float rh_peer = __shfl_xor_sync(0xffffffffu, rhv, 16);
+        const float rh_send = g1 == 0 ? rhv : rh_peer;
+        if (ok1) {
+          if ((lane & 1) == 0) {
+            if (b < nrows) {
+              const int64_t row = row0 + (int64_t)b * T;
+              a.gates[row * 3 * H + g1 * H + j1] = g;
+              if (g1 == 0) a.rh[row * H + j1] = rhv;
+            }
+            if (g1 == 1) us[b * GC_MAX_UNITS + ul] = g;
+          }
+          const uint32_t addr = gc_smem_u32(rhbuf + b * ROW + pos1);
+          gc_send(addr, bar_rh, 2 * copy1, rh_send);
+          gc_send(addr, bar_rh, 2 * copy1 + 1, rh_send);
         }
-      gc_reduce_scatter<2 * GC_RB * GC_UPW>(v, lane);
-      if ((lane & 1) == 0) {
-        const int idx = lane >> 1, gate = idx >> 3, r = (idx >> 2) & 1, u = idx & 3;
-        pre[((r0 + r) * GC_MAX_UNITS + unit0_local + u) * 2 + gate] = v[0];
       }
+      __syncwarp();
     }
-    cp_async_commit_wait_all();
-    __syncthreads();
-    GC_PROF(1);
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, j = rank * UW + ul;
-      if (b >= nrows || j >= H) continue;
-      const int64_t row = row0 + (int64_t)b * T;
-      const float* xd = xs + (b * GC_MAX_UNITS + ul) * 3;
-      const float rr = sigmoidf_(pre[(b * GC_MAX_UNITS + ul) * 2] + xd[0]);
-      const float uu = sigmoidf_(pre[(b * GC_MAX_UNITS + ul) * 2 + 1] + xd[1]);
-      const float hv = vec[b * ROW + (j / SL32) * GcGeom<CH>::SLP + (j % SL32)];
-      a.gates[row * 3 * H + j] = rr;
-      a.gates[row * 3 * H + H + j] = uu;
-      a.rh[row * H + j] = rr * hv;
-      own[(b * GC_MAX_UNITS + ul) * 2] = hv;
-      own[(b * GC_MAX_UNITS + ul) * 2 + 1] = uu;
-    }
-    GC_PROF(2);
-    cluster_barrier();
-    GC_PROF(3);
+    prof.lap(a.prof, 2);
+    gc_mbar_wait(bar_rh, step & 1);
+    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_rh, gc_phase_bytes(a));
+    prof.lap(a.prof, 3);
 
-    // ---- phase 2: c = tanh(xc + rh.Wch), h' = u*h + (1-u)*c ----
-    gc_load_vec<CH>(vec, a.rh + row0 * H, (int64_t)T * H, nrows, Bc, loader);
-    __syncthreads();
-    GC_PROF(4);
-    for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
-      float ac[GC_RB][GC_UPW];
-      gc_dot<CH>(vec, r0, lane, wc, ac);
-      float v[GC_RB * GC_UPW];  // index = row*4 + unit
+    // ---- phase 2: c = tanh(xc + rh.Wch), h' = u*h + (1-u)*c -> every CTA ----
+    if (warp_live) {
+      const uint32_t bar_next = bar_h + 8 * (par ^ 1);
+      float* hn_buf = hbuf + (par ^ 1) * Bc * ROW;
+      for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
+        float ac[GC_RB][GC_UPW];
+        gc_dot<SL>(rhbuf, r0, lane, wc, ac);
+        float v[GC_RB * GC_UPW];  // index = row*4 + unit
 #pragma unroll
-      for (int r = 0; r < GC_RB; ++r)
+        for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
-        for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = ac[r][u];
-      gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
-      if ((lane & 3) == 0) {
-        const int idx = lane >> 2, r = idx >> 2, u = idx & 3;
-        pre[((r0 + r) * GC_MAX_UNITS + unit0_local + u) * 2] = v[0];
+          for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = ac[r][u];
+        gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
+        if (!ok2) continue;
+        const int b = r0 + r2, ul = unit0_local + u2;
+        const float* xd = xc + (b * GC_MAX_UNITS + ul) * GC_XS;
+        const float c = tanhf(v[0] + xd[2]);
+        const float hv = hb[b * ROW + pos2];
+        const float uu = us[b * GC_MAX_UNITS + ul];
+        const bool live = t < lens[b];
+        float hn = live ? (uu * hv + (1.f - uu) * c) : hv;
+        const float raw = live ? hn : 0.f;
+        // the decoder feeds the DROPPED-OUT cell output back as the next state
+        if (a.drop_mask && live) hn *= xd[3];
+        if (b < nrows) {  // the four copies share the stores
+          const int64_t row = row0 + (int64_t)b * T;
+          if (copy2 == 0) a.gates[row * 3 * H + 2 * H + j2] = c;
+          else if (copy2 == 1) a.states[row * H + j2] = live ? hn : 0.f;
+          else if (copy2 == 2) { if (a.raw_states) a.raw_states[row * H + j2] = raw; }
+          else if (last) a.final_state[(int64_t)(b0 + b) * H + j2] = hn;
+          else a.hprev[((int64_t)(b0 + b) * T + t_next) * H + j2] = hn;
+        }
+        if (!last) {
+          const uint32_t addr = gc_smem_u32(hn_buf + b * ROW + pos2);
+          gc_send(addr, bar_next, 2 * copy2, hn);
+          gc_send(addr, bar_next, 2 * copy2 + 1, hn);
+        }
       }
     }
-    __syncthreads();
-    GC_PROF(5);
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, j = rank * UW + ul;
-      if (b >= nrows || j >= H) continue;
-      const int64_t row = row0 + (int64_t)b * T;
-      const float c = tanhf(pre[(b * GC_MAX_UNITS + ul) * 2] + xs[(b * GC_MAX_UNITS + ul) * 3 + 2]);
-      a.gates[row * 3 * H + 2 * H + j] = c;
-      const float hv = own[(b * GC_MAX_UNITS + ul) * 2];
-      const float uu = own[(b * GC_MAX_UNITS + ul) * 2 + 1];
-      const bool live = (a.lengths == nullptr) || (t < a.lengths[b0 + b]);
-      float hn = live ? (uu * hv + (1.f - uu) * c) : hv;
-      if (a.raw_states) a.raw_states[row * H + j] = live ? hn : 0.f;
-      if (a.drop_mask && live) hn *= a.drop_mask[row * H + j];
-      a.states[row * H + j] = live ? hn : 0.f;
-      if (last) a.final_state[(int64_t)(b0 + b) * H + j] = hn;
-      else a.hprev[((int64_t)(b0 + b) * T + t_next) * H + j] = hn;
-    }
-    GC_PROF(6);
-    cluster_barrier();
-    GC_PROF(7);
-#undef GC_PROF
+    prof.lap(a.prof, 4);
   }
+  cluster_barrier();  // no CTA leaves while a peer may still address its shared memory
 }
 
 // ---------------------------------------------------------------------------
@@ -374,134 +444,225 @@ struct GcBwdArgs {
   float* dxproj;         // [B,T,3H]
   float* dh0;            // or null
   int B, T, H, Bc, reverse;
+  long long* prof;       // optional [8] cycle counters of CTA 0 (diagnostics), or null
 };
 
-template <int CH>
+// E1: gate gradients that need no matmul, for one (row, unit): dh = carry (+ dstates, dropout,
+// + draw on live rows); returns the part of dh_prev that bypasses the matmuls (dh*u).
+// pf = the prefetched (r, u, c, h, dstates, drop mask, draw) of the item.
+__device__ __forceinline__ float gc_bwd_e1(const GcBwdArgs& a, const float* pf, float dh, bool live,
+                                           float& zc, float& zu) {
+  if (!live) {
+    zc = zu = 0.f;
+    return dh;
+  }
+  const float uu = pf[1], c = pf[2], hv = pf[3];
+  if (a.dstates) dh += pf[4];
+  if (a.drop_mask) dh *= pf[5];
+  if (a.draw) dh += pf[6];
+  const float du = dh * (hv - c);
+  const float dc = dh * (1.f - uu);
+  zc = dc * (1.f - c * c);
+  zu = du * uu * (1.f - uu);
+  return dh * uu;
+}
+
+// Asynchronous copies of step t's gates, hprev and incoming gradients of the own units, live rows
+// only, into the prefetch slot `dst` ([Bc][GC_MAX_UNITS][GC_PF]).
+__device__ __forceinline__ void gc_bwd_prefetch(const GcBwdArgs& a, int t, float* dst, const int* lens, int b0,
+                                                int ubeg, int UW) {
+  const int H = a.H, T = a.T;
+  for (int idx = threadIdx.x; idx < a.Bc * UW; idx += GC_THREADS) {
+    const int b = idx / UW, u = idx - b * UW, j = ubeg + u;
+    if (t >= lens[b]) continue;
+    const int64_t row = (int64_t)(b0 + b) * T + t;
+    float* d = dst + (b * GC_MAX_UNITS + u) * GC_PF;
+    const float* g = a.gates + row * 3 * H + j;
+    cp_async4(d, g);
+    cp_async4(d + 1, g + H);
+    cp_async4(d + 2, g + 2 * H);
+    cp_async4(d + 3, a.hprev + row * H + j);
+    if (a.dstates) cp_async4(d + 4, a.dstates + row * H + j);
+    if (a.drop_mask) cp_async4(d + 5, a.drop_mask + row * H + j);
+    if (a.draw) cp_async4(d + 6, a.draw + row * H + j);
+  }
+  cp_async_commit();
+}
+
+template <int SL>
 __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBwdArgs a) {
   extern __shared__ __align__(16) float gc_smem[];
-  constexpr int ROW = GcGeom<CH>::ROW;
+  constexpr int ROW = GcGeom<SL>::ROW;
   const int H = a.H, T = a.T, Bc = a.Bc;
-  float* vec = gc_smem;                        // [Bc][ROW]  dz_c, then dz_r
-  float* vec2 = vec + Bc * ROW;                // [Bc][ROW]  dz_u
-  float* dcarry = vec2 + Bc * ROW;             // [Bc][GC_MAX_UNITS] grad of h'_t (own units)
-  float* dhp = dcarry + Bc * GC_MAX_UNITS;     // [Bc][GC_MAX_UNITS]
-  float* pre = dhp + Bc * GC_MAX_UNITS;        // [Bc][GC_MAX_UNITS] matmul results
-  const int UW = (H + GC_CLUSTER - 1) / GC_CLUSTER;
-  const int SL32 = (H + GC_SLICES - 1) / GC_SLICES;
+  float* vc = gc_smem + GC_BAR_BYTES / 4;       // [Bc][ROW]     dz_c
+  float* vu = vc + Bc * ROW;                    // [2][Bc][ROW]  dz_u by step parity
+  float* vr = vu + 2 * Bc * ROW;                // [Bc][ROW]     dz_r
+  float* dhp = vr + Bc * ROW;                   // [Bc][GC_MAX_UNITS] part of dh_prev that bypasses the matmuls
+  float* pf = dhp + Bc * GC_MAX_UNITS;          // [2][Bc][GC_MAX_UNITS][GC_PF] by step parity
+  int* lens = reinterpret_cast<int*>(pf + 2 * Bc * GC_MAX_UNITS * GC_PF);  // [Bc]; 0 for padding rows
+  const uint32_t bar_a = gc_smem_u32(gc_smem), bar_b = bar_a + 16;     // bar_a + 8*parity: dz_c + dz_u
+  const uint32_t bytes_a = (uint32_t)(2 * Bc * H * 4), bytes_b = (uint32_t)(Bc * H * 4);
+
   const int rank = (int)cluster_rank();
+  const int ubeg = rank * H / GC_CLUSTER;      // first hidden unit of this CTA
+  const int unit_limit = (rank + 1) * H / GC_CLUSTER;
+  const int UW = unit_limit - ubeg;
   const int b0 = (blockIdx.x / GC_CLUSTER) * Bc;
   const int nrows = min(Bc, a.B - b0);
-  const GcLoader loader = gc_make_loader<CH>(H, SL32);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int unit0_local = warp * GC_UPW;
-  const int unit0 = rank * UW + unit0_local;   // first OUTPUT unit i of this warp
-  const int unit_limit = min(H, (rank + 1) * UW);
+  const int unit0 = ubeg + unit0_local;        // first OUTPUT unit i of this warp
+  const bool warp_live = unit0 < unit_limit;
 
   // rows i of Wch / Wgh restricted to this lane's slice of the reduction index j
-  float w1[GC_UPW][4 * CH], w2r[GC_UPW][4 * CH], w2u[GC_UPW][4 * CH];
-  gc_load_w<CH>(w1, a.Wch, 1, H, unit0, H, unit_limit, lane * SL32, SL32, H);
-  gc_load_w<CH>(w2r, a.Wgh, 1, 2 * H, unit0, H, unit_limit, lane * SL32, SL32, H);
-  gc_load_w<CH>(w2u, a.Wgh + H, 1, 2 * H, unit0, H, unit_limit, lane * SL32, SL32, H);
+  float w1[GC_UPW][SL], w2r[GC_UPW][SL], w2u[GC_UPW][SL];
+  gc_load_w<SL>(w1, a.Wch, 1, H, unit0, unit_limit, lane * SL, H);
+  gc_load_w<SL>(w2r, a.Wgh, 1, 2 * H, unit0, unit_limit, lane * SL, H);
+  gc_load_w<SL>(w2u, a.Wgh + H, 1, 2 * H, unit0, unit_limit, lane * SL, H);
 
-  for (int i = threadIdx.x; i < 2 * Bc * ROW; i += GC_THREADS) vec[i] = 0.f;  // incl. vec2; see fwd
-  for (int idx = threadIdx.x; idx < Bc * GC_MAX_UNITS; idx += GC_THREADS) {
-    const int b = idx / GC_MAX_UNITS, ul = idx - b * GC_MAX_UNITS, j = rank * UW + ul;
-    dcarry[idx] = (a.dfinal && b < nrows && ul < UW && j < H) ? a.dfinal[(int64_t)(b0 + b) * H + j] : 0.f;
+  // the (row, unit) this lane holds after a reduce-scatter of 8 values, and its copy index
+  const int rr_ = (lane >> 4) & 1, uq = (lane >> 2) & 3, copy = lane & 3;
+  const bool ok = unit0 + uq < unit_limit;
+  const int ji = unit0 + uq, ul = unit0_local + uq;
+  const int pos = ok ? GcGeom<SL>::pos(ji) : 0;
+  // time of the k-th step processed
+  auto time_of = [reverse = a.reverse, T](int k) { return reverse ? k : T - 1 - k; };
+
+  if (threadIdx.x == 0) {
+    gc_mbar_init(bar_a);
+    gc_mbar_init(bar_a + 8);
+    gc_mbar_init(bar_b);
+    gc_mbar_arm(bar_a, bytes_a);
+    gc_mbar_arm(bar_a + 8, bytes_a);
+    gc_mbar_arm(bar_b, bytes_b);
   }
+  for (int i = threadIdx.x; i < 4 * Bc * ROW; i += GC_THREADS) vc[i] = 0.f;  // vc, vu, vr; see fwd
+  for (int i = threadIdx.x; i < 2 * Bc * GC_MAX_UNITS * GC_PF; i += GC_THREADS) pf[i] = 0.f;
+  for (int b = threadIdx.x; b < Bc; b += GC_THREADS)
+    lens[b] = b < nrows ? (a.lengths ? a.lengths[b0 + b] : T) : 0;
   __syncthreads();
 
-  for (int step = T - 1; step >= 0; --step) {
-    const int t = a.reverse ? T - 1 - step : step;
+
+  gc_bwd_prefetch(a, time_of(0), pf, lens, b0, ubeg, UW);
+  cp_async_wait_all();
+  __syncthreads();
+  cluster_barrier();  // every CTA's barriers are initialised and its buffers zeroed before anyone sends
+  {  // E1 of the first step processed, from dfinal
+    const int t = time_of(0);
+    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
+      const int b = idx / UW, u = idx - b * UW, j = ubeg + u;
+      const bool live = t < lens[b];
+      const float dh = (a.dfinal && b < nrows) ? a.dfinal[(int64_t)(b0 + b) * H + j] : 0.f;
+      float zc, zu;
+      dhp[b * GC_MAX_UNITS + u] = gc_bwd_e1(a, pf + (b * GC_MAX_UNITS + u) * GC_PF, dh, live, zc, zu);
+      if (b < nrows) {
+        const int64_t row = (int64_t)(b0 + b) * T + t;
+        a.dxproj[row * 3 * H + H + j] = zu;
+        a.dxproj[row * 3 * H + 2 * H + j] = zc;
+      }
+      const int p = GcGeom<SL>::pos(j);
+      const uint32_t ac = gc_smem_u32(vc + b * ROW + p), au = gc_smem_u32(vu + b * ROW + p);
+      for (int d = 0; d < GC_CLUSTER; ++d) {
+        gc_send(ac, bar_a, d, zc);
+        gc_send(au, bar_a, d, zu);
+      }
+    }
+  }
+
+  GcProf prof(a.prof);
+  for (int k = 0; k < T; ++k) {
+    const int t = time_of(k);
+    const bool last = (k == T - 1);
     const int64_t row0 = (int64_t)b0 * T + t;
-    // ---- E1: gate gradients that need no matmul (own units) ----
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, j = rank * UW + ul;
-      if (b >= nrows || j >= H) continue;
-      const int64_t row = row0 + (int64_t)b * T;
-      const bool live = (a.lengths == nullptr) || (t < a.lengths[b0 + b]);
-      float dh = dcarry[b * GC_MAX_UNITS + ul];
-      if (!live) {
-        a.dxproj[row * 3 * H + j] = 0.f;
-        a.dxproj[row * 3 * H + H + j] = 0.f;
-        a.dxproj[row * 3 * H + 2 * H + j] = 0.f;
-        dhp[b * GC_MAX_UNITS + ul] = dh;
-        continue;
+    const int par = k & 1;
+    const float* pfc = pf + par * Bc * GC_MAX_UNITS * GC_PF;
+    float* pfn = pf + (par ^ 1) * Bc * GC_MAX_UNITS * GC_PF;
+
+    gc_mbar_wait(bar_a + 8 * par, (k >> 1) & 1);
+    if (threadIdx.x == 0 && k + 2 < T) gc_mbar_arm(bar_a + 8 * par, bytes_a);
+    prof.lap(a.prof, 0);
+    __syncthreads();  // every warp is done with the previous step (and its prefetch slot)
+    if (!last) gc_bwd_prefetch(a, time_of(k + 1), pfn, lens, b0, ubeg, UW);
+    prof.lap(a.prof, 1);
+
+    // ---- G1: drh = dz_c . Wch^T ; dz_r = drh*h*r*(1-r) ; dhp += drh*r -> dz_r to every CTA ----
+    if (warp_live) {
+      for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
+        float acc[GC_RB][GC_UPW];
+        gc_dot<SL>(vc, r0, lane, w1, acc);
+        float v[GC_RB * GC_UPW];
+#pragma unroll
+        for (int r = 0; r < GC_RB; ++r)
+#pragma unroll
+          for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = acc[r][u];
+        gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
+        if (!ok) continue;
+        const int b = r0 + rr_;
+        const float drh = v[0];
+        const bool live = t < lens[b];
+        const float* s = pfc + (b * GC_MAX_UNITS + ul) * GC_PF;
+        const float rg = s[0], hv = s[3];
+        const float zr = live ? drh * hv * rg * (1.f - rg) : 0.f;
+        if (copy == 0) {
+          if (b < nrows) a.dxproj[(row0 + (int64_t)b * T) * 3 * H + ji] = zr;
+          if (live) dhp[b * GC_MAX_UNITS + ul] += drh * rg;
+        }
+        const uint32_t addr = gc_smem_u32(vr + b * ROW + pos);
+        gc_send(addr, bar_b, 2 * copy, zr);
+        gc_send(addr, bar_b, 2 * copy + 1, zr);
       }
-      const float uu = a.gates[row * 3 * H + H + j], c = a.gates[row * 3 * H + 2 * H + j];
-      const float hv = a.hprev[row * H + j];
-      if (a.dstates) dh += a.dstates[row * H + j];
-      if (a.drop_mask) dh *= a.drop_mask[row * H + j];
-      if (a.draw) dh += a.draw[row * H + j];
-      const float du = dh * (hv - c);
-      const float dc = dh * (1.f - uu);
-      a.dxproj[row * 3 * H + 2 * H + j] = dc * (1.f - c * c);
-      a.dxproj[row * 3 * H + H + j] = du * uu * (1.f - uu);
-      dhp[b * GC_MAX_UNITS + ul] = dh * uu;
+      __syncwarp();
     }
-    cluster_barrier();
-    // ---- G1: drh = dz_c . Wch^T ; dz_r = drh*h*r*(1-r) ; dhp += drh*r ----
-    gc_load_vec<CH>(vec, a.dxproj + row0 * 3 * H + 2 * H, (int64_t)T * 3 * H, nrows, Bc, loader);
-    gc_load_vec<CH>(vec2, a.dxproj + row0 * 3 * H + H, (int64_t)T * 3 * H, nrows, Bc, loader);
-    __syncthreads();
-    for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
-      float acc[GC_RB][GC_UPW];
-      gc_dot<CH>(vec, r0, lane, w1, acc);
-      float v[GC_RB * GC_UPW];
+    prof.lap(a.prof, 2);
+    gc_mbar_wait(bar_b, k & 1);
+    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_b, bytes_b);
+    prof.lap(a.prof, 3);
+    cp_async_wait_all();
+    __syncthreads();  // the next step's prefetch is in
+    prof.lap(a.prof, 4);
+
+    // ---- G2: dcarry = dhp + [dz_r, dz_u] . Wgh^T, then E1 of the next step -> dz_c, dz_u ----
+    if (warp_live) {
+      const float* vuc = vu + par * Bc * ROW;
+      const int tn = last ? t : time_of(k + 1);
+      for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
+        float accr[GC_RB][GC_UPW], accu[GC_RB][GC_UPW];
+        gc_dot<SL>(vr, r0, lane, w2r, accr);
+        gc_dot<SL>(vuc, r0, lane, w2u, accu);
+        float v[GC_RB * GC_UPW];
 #pragma unroll
-      for (int r = 0; r < GC_RB; ++r)
+        for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
-        for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = acc[r][u];
-      gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
-      if ((lane & 3) == 0) {
-        const int idx = lane >> 2, r = idx >> 2, u = idx & 3;
-        pre[(r0 + r) * GC_MAX_UNITS + unit0_local + u] = v[0];
+          for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = accr[r][u] + accu[r][u];
+        gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
+        const int b = r0 + rr_;
+        const float dcarry = ok ? dhp[b * GC_MAX_UNITS + ul] + v[0] : 0.f;
+        __syncwarp();  // every copy has read dhp before copy 0 replaces it
+        if (!ok) continue;
+        if (last) {
+          if (a.dh0 && copy == 0 && b < nrows) a.dh0[(int64_t)(b0 + b) * H + ji] = dcarry;
+          continue;
+        }
+        float zc, zu;
+        const float d = gc_bwd_e1(a, pfn + (b * GC_MAX_UNITS + ul) * GC_PF, dcarry, tn < lens[b], zc, zu);
+        if (b < nrows) {
+          const int64_t row = (int64_t)(b0 + b) * T + tn;
+          if (copy == 1) a.dxproj[row * 3 * H + H + ji] = zu;
+          else if (copy == 2) a.dxproj[row * 3 * H + 2 * H + ji] = zc;
+        }
+        if (copy == 0) dhp[b * GC_MAX_UNITS + ul] = d;
+        const uint32_t ac = gc_smem_u32(vc + b * ROW + pos);
+        const uint32_t au = gc_smem_u32(vu + ((par ^ 1) * Bc + b) * ROW + pos);
+        const uint32_t bar_next = bar_a + 8 * (par ^ 1);
+        gc_send(ac, bar_next, 2 * copy, zc);
+        gc_send(ac, bar_next, 2 * copy + 1, zc);
+        gc_send(au, bar_next, 2 * copy, zu);
+        gc_send(au, bar_next, 2 * copy + 1, zu);
       }
     }
-    __syncthreads();
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, i = rank * UW + ul;
-      if (b >= nrows || i >= H) continue;
-      const bool live = (a.lengths == nullptr) || (t < a.lengths[b0 + b]);
-      if (!live) continue;
-      const int64_t row = row0 + (int64_t)b * T;
-      const float drh = pre[b * GC_MAX_UNITS + ul];
-      const float rr = a.gates[row * 3 * H + i];
-      const float hv = a.hprev[row * H + i];
-      a.dxproj[row * 3 * H + i] = drh * hv * rr * (1.f - rr);
-      dhp[b * GC_MAX_UNITS + ul] += drh * rr;
-    }
-    cluster_barrier();
-    // ---- G2: dcarry = dhp + [dz_r, dz_u] . Wgh^T ----
-    gc_load_vec<CH>(vec, a.dxproj + row0 * 3 * H, (int64_t)T * 3 * H, nrows, Bc, loader);
-    __syncthreads();
-    for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
-      float accr[GC_RB][GC_UPW], accu[GC_RB][GC_UPW];
-      gc_dot<CH>(vec, r0, lane, w2r, accr);
-      gc_dot<CH>(vec2, r0, lane, w2u, accu);
-      float v[GC_RB * GC_UPW];
-#pragma unroll
-      for (int r = 0; r < GC_RB; ++r)
-#pragma unroll
-        for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = accr[r][u] + accu[r][u];
-      gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
-      if ((lane & 3) == 0) {
-        const int idx = lane >> 2, r = idx >> 2, u = idx & 3;
-        pre[(r0 + r) * GC_MAX_UNITS + unit0_local + u] = v[0];
-      }
-    }
-    __syncthreads();
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW;
-      dcarry[b * GC_MAX_UNITS + ul] = dhp[b * GC_MAX_UNITS + ul] + pre[b * GC_MAX_UNITS + ul];
-    }
-    __syncthreads();  // dcarry/dhp/pre/vec are CTA-private: no cluster barrier needed here
+    prof.lap(a.prof, 5);
   }
-  if (a.dh0) {
-    for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-      const int b = idx / UW, ul = idx - b * UW, j = rank * UW + ul;
-      if (b < nrows && j < H) a.dh0[(int64_t)(b0 + b) * H + j] = dcarry[b * GC_MAX_UNITS + ul];
-    }
-  }
+  cluster_barrier();  // no CTA leaves while a peer may still address its shared memory
 }
 
 }  // namespace nm

@@ -574,9 +574,9 @@ def gru_layer(x: torch.Tensor, gates_kernel: torch.Tensor, gates_bias: torch.Ten
 
 
 class _BiGRULayer(torch.autograd.Function):
-    """Forward and backward direction of a bidirectional GRU layer over the same input, their recurrences
-    in ONE launch each way (nm_gru_seq_fwd_pair / nm_gru_seq_bwd_pair): the two directions are
-    independent, and one direction alone occupies only half of the SMs for T dependent steps."""
+    """Forward and backward direction of a bidirectional GRU layer over the same input.  Their recurrences
+    go through one entry point each way (nm_gru_seq_fwd_pair / nm_gru_seq_bwd_pair), which runs the two
+    directions one after the other, each on the whole GPU."""
 
     @staticmethod
     def forward(ctx, x, lengths, wg_f, bg_f, wc_f, bc_f, wg_b, bg_b, wc_b, bc_b):
