@@ -259,7 +259,7 @@ int nm_logits_xent_bwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
                        float* dlogits, int64_t ldd, int64_t M, int64_t V,
                        int64_t K, void* stream);
 
-/* ---- K5/K6 with fp16 operands (fp16 operands), optional path - ops.py uses it with NMB200_XENT16=1 ----
+/* ---- K5/K6 with fp16 operands: the default path of ops.logits_xent (NMB200_XENT16=0 selects TF32) ----
  * Every product is K-major x K-major: X16 [M,K], WT16 [V,K] (the projection matrix transposed),
  * row pitches multiples of 8 elements, bases 16-byte aligned.
  * nm_cast_f16: dst = half(src * row_scale[row]) (row_scale may be NULL) followed by `extra_ones` columns
@@ -268,8 +268,9 @@ int nm_logits_xent_bwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
  * nm_gemm_f16: C[M,N] (or C^T when transposed != 0: element (m,n) -> C[n*ldc+m])
  *   = alpha_dev[0] * row_scale[m] * A16[M,K] . B16[N,K]^T  (+ C when beta == 1).
  * nm_logits_xent_fwd16: as nm_logits_xent_fwd.
- * nm_logits_xent_bwd16: dl16 [M,V] (and dlT16 [V,M] unless NULL) = half((softmax - onehot) * mask[m]);
- *   the upstream scale is applied by the consumers (replaces autoregressive.py:292-316 backward). */
+ * nm_logits_xent_bwd16: dl16 [M,V] = half((softmax - onehot) * mask[m]), row pitch ldd (a multiple of 8,
+ *   base 16-byte aligned); the upstream scale is applied by the consumers (replaces autoregressive.py:292-316
+ *   backward). */
 int nm_cast_f16(const float* src, int64_t ld_src, void* dst, int64_t ld_dst, int64_t rows,
                 int64_t cols, const float* row_scale, int transpose, int extra_ones, void* stream);
 int nm_gemm_f16(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16,
@@ -287,8 +288,7 @@ int nm_logits_xent_fwd16(const void* X16, int64_t ldx, const void* WT16, int64_t
                          int64_t M, int64_t V, int64_t K, void* stream);
 int nm_logits_xent_bwd16(const void* X16, int64_t ldx, const void* WT16, int64_t ldw, const float* b,
                          int64_t unk_index, const int64_t* targets, const float* mask, const float* lse,
-                         void* dl16, int64_t ldd, void* dlT16, int64_t lddt, int64_t M, int64_t V,
-                         int64_t K, void* stream);
+                         void* dl16, int64_t ldd, int64_t M, int64_t V, int64_t K, void* stream);
 
 /* ---- K11: beam-search step ----------------------------------------------------
  * Replaces steps (1)-(8) of BeamSearchDecoder body

@@ -61,17 +61,6 @@ struct RowStats {
   int32_t arg;
 };
 
-constexpr float TC_LOG2E = 1.4426950408889634f;
-
-// 2^x as ONE MUFU instruction.  exp2f() wraps the same MUFU.EX2 in a range fix for results below 2^-126
-// (compare, halve, square: three more issue slots per element in epilogues that run once per logit); here such
-// results flush to zero, which is what they contribute to a sum of probabilities anyway.
-__device__ __forceinline__ float fast_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 __device__ __forceinline__ void load_bias32(const float* __restrict__ bias, int col0, int ncols,
                                             float (&b)[32]) {
   if (bias == nullptr) {
@@ -274,19 +263,14 @@ __device__ __forceinline__ void epilogue_chunk_atomic(const TcEpilogue& e, const
 // ---------------------------------------------------------------------------
 // Transposed store of a warp's 32x32 chunk: lane = row, so for one column the 32 lanes write 32
 // consecutive elements of the transposed matrix - a full segment without any staging.
-template <typename T>
-__device__ __forceinline__ void store32_transposed(T* __restrict__ ct, int64_t ldt, int64_t row, int col0,
+__device__ __forceinline__ void store32_transposed(float* __restrict__ ct, int64_t ldt, int64_t row, int col0,
                                                    int64_t M, int ncols, const float (&x)[32], float beta) {
   if (row >= M) return;
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     if (j < ncols) {
-      T* dst = ct + (int64_t)(col0 + j) * ldt + row;
-      if constexpr (sizeof(T) == 2) {
-        *dst = __float2half_rn(x[j]);
-      } else {
-        *dst = (beta != 0.f) ? (x[j] + *dst) : x[j];
-      }
+      float* dst = ct + (int64_t)(col0 + j) * ldt + row;
+      *dst = (beta != 0.f) ? (x[j] + *dst) : x[j];
     }
   }
 }
@@ -318,7 +302,7 @@ __device__ __forceinline__ void store32_half_coalesced(float* __restrict__ stage
   __syncwarp();
 }
 
-// TC_EPI_XENT_BWD16: (softmax - onehot) * row weight, stored as fp16 row-major and transposed.
+// TC_EPI_XENT_BWD16: (softmax - onehot) * row weight, stored as fp16 row-major.
 // The row weight is the 0/1 mask here (the caller applies the upstream scale in the consumers), so
 // the stored values lie in [-1, 1] and fp16 keeps TF32's 10 mantissa bits for them.
 __device__ __forceinline__ void epilogue_chunk_xent_bwd16(const TcEpilogue& e, const TcExt& ext, float (&x)[32],
@@ -354,8 +338,6 @@ __device__ __forceinline__ void epilogue_chunk_xent_bwd16(const TcEpilogue& e, c
     for (int j = 0; j < 32; ++j)
       if (j < ncols) c16[row * ext.ldc16 + col0 + j] = __float2half_rn(x[j]);
   }
-  if (ext.C16T)
-    store32_transposed(reinterpret_cast<__half*>(ext.C16T), ext.ldc16t, row, col0, M, ncols, x, 0.f);
 }
 
 // TC_EPI_DENSE of the fp16 instances: C (or C^T) = alpha * row_scale[m] * acc + bias (+ C).
@@ -821,9 +803,7 @@ static int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t c
   return NM_OK;
 }
 
-// 2-D fp16 tensor [rows, cols] with row pitch ld (elements), K-major operand tile: box = {64 elements of K,
-// box_rows}, 128-byte swizzle.
-static int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
+int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld,
                       uint32_t box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   NM_REQUIRE(fn != nullptr, NM_E_NO_DEVICE, "tc_gemm16: cuTensorMapEncodeTiled not available");

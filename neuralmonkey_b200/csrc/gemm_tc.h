@@ -1,5 +1,6 @@
 // Host interface of the wgmma GEMM (gemm_tc.cu).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -9,7 +10,7 @@ enum TcEpiMode {
   TC_EPI_DENSE = 0,     // C = act(acc + bias) + beta*C
   TC_EPI_XENT_FWD = 1,  // per-(row, n-tile) softmax partials; optional logits store
   TC_EPI_XENT_BWD = 2,  // C = (exp(x - lse) - onehot) * weights * scale
-  TC_EPI_XENT_BWD16 = 3,  // fp16 operands: C16 (and C16T) = half((exp(x - lse) - onehot) * weights)
+  TC_EPI_XENT_BWD16 = 3,  // fp16 operands: C16 = half((exp(x - lse) - onehot) * weights)
   TC_EPI_SOFTMAX = 4,   // batched attention energies: C = softmax(mask(acc * scale)) (and C2 = C * drop)
   TC_EPI_DSOFTMAX = 5,  // batched: C = scale * mask' * P * (acc * drop - sum_j(acc * drop * P))
 };
@@ -38,8 +39,6 @@ struct TcEpilogue {
 struct TcExt {
   void* C16;               // xent_bwd16: [M,N] fp16, row pitch ldc16 (elements)
   int64_t ldc16;
-  void* C16T;              // xent_bwd16: the same matrix transposed, [N,M] fp16, row pitch ldc16t; may be null
-  int64_t ldc16t;
   const float* alpha;      // dense: device scalar multiplying the accumulator (null: 1)
   const float* row_scale;  // dense: [M] per-row factor (null: 1)
   int transposed;          // dense: store D^T - element (m, n) goes to C[n * ldc + m]
@@ -72,6 +71,22 @@ struct TcBatch {
 int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t a_rows,
                            int64_t a_cols, int64_t lda, const float* B, int64_t b_rows, int64_t b_cols,
                            int64_t ldb, const TcEpilogue& epi, const TcBatch& bt, cudaStream_t s);
+
+// 2-D fp16 tensor [rows, cols] with row pitch ld (elements), K-major operand tile: box = {64 elements of K,
+// box_rows}, 128-byte swizzle; elements outside [rows, cols] load as zeros.
+int make_map16(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld, uint32_t box_rows);
+
+// The persistent fp16 vocabulary cross-entropy kernel (xent16.cu) for K <= XENT16_MAX_K:
+// X16 [M,K] . WT16 [V,K]^T + b with
+//   bwd = false: softmax partials into part ([M][2*ceil(V/TC_XENT_BN)] float4, see TcEpilogue::part) and the
+//                logits into logits_out (fp32, row pitch ldl) unless it is null;
+//   bwd = true:  dl16 [M,V] (fp16, row pitch ldd) = (softmax - onehot(targets)) * mask, with softmax from lse.
+// Longer K runs the TC_EPI_XENT_FWD / TC_EPI_XENT_BWD16 instances of tc_gemm16_launch.
+constexpr int64_t XENT16_MAX_K = 320;
+int xent16_launch(bool bwd, const void* X16, int64_t ldx, const void* WT16, int64_t ldw, const float* b,
+                  int64_t unk_index, const int64_t* targets, const float* mask, const float* lse, float4* part,
+                  float* logits_out, int64_t ldl, void* dl16, int64_t ldd, int64_t M, int64_t V, int64_t K,
+                  cudaStream_t s);
 
 // True when the operands can be addressed by TMA (16-byte aligned rows and bases).
 bool tc_gemm_supported(int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, const void* A, const void* B);

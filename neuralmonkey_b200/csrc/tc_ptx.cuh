@@ -49,6 +49,17 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+constexpr float TC_LOG2E = 1.4426950408889634f;
+
+// 2^x as ONE MUFU instruction.  exp2f() wraps the same MUFU.EX2 in a range fix for results below 2^-126
+// (compare, halve, square: three more issue slots per element in epilogues that run once per logit); here such
+// results flush to zero, which is what they contribute to a sum of probabilities anyway.
+__device__ __forceinline__ float fast_ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));

@@ -116,16 +116,24 @@ int nm_logits_xent_fwd16(const void* X16, int64_t ldx, const void* WT16, int64_t
   NM_REQUIRE(X16 && WT16 && lse && part, NM_E_INVALID, "nm_logits_xent_fwd16: null pointer");
   NM_REQUIRE(M > 0 && V > 0 && K > 0 && ldx >= K && ldw >= K, NM_E_INVALID, "nm_logits_xent_fwd16: bad sizes");
   NM_REQUIRE(!logits_out || ldl >= V, NM_E_INVALID, "nm_logits_xent_fwd16: ldl < V");
+  NM_REQUIRE((reinterpret_cast<uintptr_t>(part) & 15) == 0, NM_E_INVALID,
+             "nm_logits_xent_fwd16: part must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
-  TcEpilogue epi{};
-  epi.mode = TC_EPI_XENT_FWD;
-  epi.C = logits_out;
-  epi.ldc = ldl;
-  epi.bias = b;
-  epi.unk_index = unk_index;
-  epi.targets = targets;
-  epi.part = reinterpret_cast<float4*>(part);
-  const int rc = tc_gemm16_launch(M, V, K, X16, ldx, WT16, ldw, epi, TcExt{}, s);
+  int rc;
+  if (K <= XENT16_MAX_K) {
+    rc = xent16_launch(false, X16, ldx, WT16, ldw, b, unk_index, targets, nullptr, nullptr,
+                       reinterpret_cast<float4*>(part), logits_out, ldl, nullptr, 0, M, V, K, s);
+  } else {
+    TcEpilogue epi{};
+    epi.mode = TC_EPI_XENT_FWD;
+    epi.C = logits_out;
+    epi.ldc = ldl;
+    epi.bias = b;
+    epi.unk_index = unk_index;
+    epi.targets = targets;
+    epi.part = reinterpret_cast<float4*>(part);
+    rc = tc_gemm16_launch(M, V, K, X16, ldx, WT16, ldw, epi, TcExt{}, s);
+  }
   if (rc) return rc;
   const int64_t tiles_n = 2 * ceil_div(V, TC_XENT_BN);
   xent_combine_kernel<<<(unsigned)ceil_div(M, 8), 256, 0, s>>>(reinterpret_cast<const float4*>(part), M,

@@ -820,7 +820,7 @@ class _LogitsXent16(torch.autograd.Function):
         # (softmax - onehot) * mask in fp16, row-major; values in [-1, 1]
         dl16 = torch.empty(m, vpad, device=dev, dtype=torch.float16)
         call("nm_logits_xent_bwd16", ptr(x16), kpad, ptr(wt16), kpad, ptr(b), unk_index, ptr(targets),
-             ptr(weights), ptr(lse), ptr(dl16), vpad, None, 0, m, v, k, lib.stream())
+             ptr(weights), ptr(lse), ptr(dl16), vpad, m, v, k, lib.stream())
         upstream = dxent.reshape(-1).to(torch.float32).contiguous()    # per-row factor, applied in fp32
         dx = None
         if ctx.needs_input_grad[0]:
