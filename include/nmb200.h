@@ -158,9 +158,6 @@ int nm_gru_seq_fwd(const float* xproj, const float* Wgh, const float* Wch,
 /* Number of 8-CTA clusters of the persistent GRU kernel that are co-resident on the
  * current device (forward: backward=0).  Diagnostic. */
 int nm_gru_resident_clusters(int backward);
-/* Recurrence engine of nm_gru_seq_fwd/bwd: 0 (default) or 1; on sm_90a both run the persistent cluster
- * kernels in exact fp32 (the mode is recorded for callers that set it). */
-int nm_gru_set_mode(int mode);
 /* Diagnostic: 8 int64 device counters receiving the cycles thread 0 of CTA 0 of the forward and
  * backward cluster kernels spends per section of a step (see tools/gru_probe.py). NULL = off. */
 int nm_gru_debug_profile(void* counters);
@@ -259,7 +256,7 @@ int nm_logits_xent_bwd(const float* X, int64_t ldx, const float* W, int64_t ldw,
                        float* dlogits, int64_t ldd, int64_t M, int64_t V,
                        int64_t K, void* stream);
 
-/* ---- K5/K6 with fp16 operands: the default path of ops.logits_xent (NMB200_XENT16=0 selects TF32) ----
+/* ---- K5/K6 with fp16 operands: the default path of ops.logits_xent ----
  * Every product is K-major x K-major: X16 [M,K], WT16 [V,K] (the projection matrix transposed),
  * row pitches multiples of 8 elements, bases 16-byte aligned.
  * nm_cast_f16: dst = half(src * row_scale[row]) (row_scale may be NULL) followed by `extra_ones` columns

@@ -18,7 +18,6 @@ from neuralmonkey_b200.decorators import tensor
 from neuralmonkey_b200.model.model_part import ModelPart
 from neuralmonkey_b200.model.parameterized import InitializerSpecs
 from neuralmonkey_b200.nn.utils import dropout, dropout_mask
-from neuralmonkey_b200.nn.variants import require_variant
 from neuralmonkey_b200.params import variance_scaling_initializer, zeros_initializer
 from neuralmonkey_b200.typecheck import check_argument_types
 
@@ -62,7 +61,6 @@ def attention(part, scope: str, queries: torch.Tensor, keys: torch.Tensor, value
     drop = None
     if attention_dropout_keep_prob < 1.0 and train_mode:
         # dropout on the attention weights (:208-214), inside the fused core: the mask rides along
-        require_variant("attention_dropout_keep_prob < 1")
         drop = dropout_mask((queries.shape[0], num_heads, queries.shape[1], keys.shape[1]),
                             attention_dropout_keep_prob, train_mode, queries.device)
     context, weights = ops.mha_core(queries, keys, values, keys_mask, masked, num_heads, drop)

@@ -19,7 +19,6 @@
 // Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" of the wgmma section.
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -615,11 +614,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  // Programmatic dependent launch (NMB200_TC_PDL): the barrier set-up above touches no global memory and may run
-  // while the previous kernel of the stream drains; from here on its results are needed.  Without the launch
-  // attribute both instructions do nothing.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   if (warp < 4) {
     // ===================== producer warpgroup =====================
@@ -839,16 +833,6 @@ bool tc_gemm_supported(int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb
   return true;
 }
 
-// NMB200_TC_PDL=1: launch with programmatic stream serialization, so that a kernel's prologue overlaps the tail of
-// its predecessor (the kernel waits with griddepcontrol.wait before it touches global memory)
-static bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("NMB200_TC_PDL");
-    return e && atoi(e) != 0;
-  }();
-  return on;
-}
-
 // one CTA per work item (tile x split-K slice, or tile x batched problem)
 template <int BN, bool A_MN, bool B_MN, int MODE, int ESZ>
 static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
@@ -869,13 +853,6 @@ static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOp
   cfg.blockDim = dim3(TC_THREADS);
   cfg.dynamicSmemBytes = (size_t)Cfg::SMEM_BYTES;
   cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
   NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt));
   NM_LAUNCH_CHECK(name);
   return NM_OK;

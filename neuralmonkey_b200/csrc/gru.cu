@@ -9,9 +9,6 @@
 // Each step is two fused GEMM+gate kernels forward and one gate kernel plus two
 // fused GEMM kernels backward; the state the step consumed is read from / written
 // to the `hprev` history directly, so no state copy kernels are launched.
-#include <stdlib.h>
-#include <string.h>
-
 #include "gemm_simt.cuh"
 #include "gru_cluster.cuh"
 
@@ -132,17 +129,8 @@ using namespace nm;
 namespace {
 
 // Persistent cluster kernels need the three weight vectors of a unit slice in registers:
-// H <= 320.  NMB200_GRU=steps forces the per-step kernels (debugging / A-B timing).
-bool cluster_path_ok(int64_t H) {
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("NMB200_GRU");
-    forced = (e && strcmp(e, "steps") == 0) ? 1 : 0;
-  }
-  return forced == 0 && H >= 8 && H <= 320;
-}
-
-int g_gru_mode = 0;   // nm_gru_set_mode(): recorded; every mode runs the cluster engine on sm_90a
+// H <= 320.  Other widths run on the per-step kernels.
+bool cluster_path_ok(int64_t H) { return H >= 8 && H <= 320; }
 
 struct ClusterPlan {
   int Bc, nclusters, sl;
@@ -241,12 +229,6 @@ int launch_cluster(Kern kern, const Args& args, const ClusterPlan& p, cudaStream
 extern "C" {
 
 int nm_gru_resident_clusters(int backward) { return resident_clusters(backward != 0); }
-
-int nm_gru_set_mode(int mode) {
-  NM_REQUIRE(mode == 0 || mode == 1, NM_E_INVALID, "nm_gru_set_mode: mode must be 0 (tensor cores) or 1 (exact fp32)");
-  g_gru_mode = mode;
-  return NM_OK;
-}
 
 static long long* g_gru_prof = nullptr;
 /* Diagnostic: device buffer of 8 int64 cycle counters accumulated by thread 0 of CTA 0 of the next

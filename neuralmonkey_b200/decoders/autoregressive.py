@@ -65,9 +65,6 @@ class AutoregressiveDecoder(ModelPart):
             raise ValueError("Embedding size must be a positive integer.")
         if self.dropout_keep_prob < 0.0 or self.dropout_keep_prob > 1.0:
             raise ValueError("Dropout keep probability must be a real number in the interval [0,1].")
-        if self.label_smoothing:
-            from neuralmonkey_b200.nn.variants import require_variant
-            require_variant("label_smoothing")
         self._train_ids_host = None  # type: Optional[torch.Tensor]
 
     # -- static configuration ----------------------------------------------------------

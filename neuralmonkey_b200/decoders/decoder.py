@@ -32,7 +32,7 @@ from neuralmonkey_b200.model.parameterized import InitializerSpecs
 from neuralmonkey_b200.model.sequence import EmbeddedSequence
 from neuralmonkey_b200.model.stateful import Stateful
 from neuralmonkey_b200.nn.utils import dropout, dropout_mask
-from neuralmonkey_b200.nn.variants import LSTMCell, NematusGRUCell, require_variant
+from neuralmonkey_b200.nn.variants import LSTMCell, NematusGRUCell
 from neuralmonkey_b200.vocabulary import Vocabulary
 
 RNN_CELL_TYPES = ("NematusGRU", "GRU", "LSTM")
@@ -84,8 +84,6 @@ class Decoder(AutoregressiveDecoder):
             raise NotImplementedError("attention_on_input=True fails in the reference while the graph is "
                                       "built (decoders/decoder.py:273); it is not supported here either")
         self._stepwise = self._rnn_cell_str != "GRU" or conditional_gru
-        if self._stepwise:
-            require_variant("Decoder with rnn_cell='{}', conditional_gru={}".format(rnn_cell, conditional_gru))
         for att in self.attentions:
             if hasattr(att, "set_query_size"):
                 att.set_query_size(self.rnn_size)

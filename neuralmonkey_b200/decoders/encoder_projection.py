@@ -11,7 +11,6 @@ import torch
 from neuralmonkey_b200 import ops, runtime
 from neuralmonkey_b200.model.stateful import Stateful
 from neuralmonkey_b200.nn.utils import dropout
-from neuralmonkey_b200.nn.variants import require_variant
 from neuralmonkey_b200.params import block_orthogonal_initializer, zeros_initializer
 
 
@@ -126,5 +125,4 @@ class _Nematus(EncoderProjection):
 def nematus_projection(dropout_keep_prob: float = 1.0) -> EncoderProjection:
     """tanh(dense(mean of the encoder's states over its unmasked positions))
     (encoder_projection.py:99-145)."""
-    require_variant("nematus_projection")
     return _Nematus(dropout_keep_prob)

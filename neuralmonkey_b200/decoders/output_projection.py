@@ -10,7 +10,6 @@ import torch
 
 from neuralmonkey_b200 import ops
 from neuralmonkey_b200.nn.utils import dropout
-from neuralmonkey_b200.nn.variants import require_variant
 from neuralmonkey_b200.params import zeros_initializer
 
 
@@ -130,12 +129,10 @@ def _activation_name(activation_fn) -> str:
 def nematus_output(output_size: int, activation_fn: str = "tanh",
                    dropout_keep_prob: float = 1.0) -> Tuple[OutputProjection, int]:
     """activation(dense(state) + dense(embedding) + dense(contexts)) (output_projection.py:76-112)."""
-    require_variant("nematus_output")
     return _Nematus(output_size, _activation_name(activation_fn), dropout_keep_prob), output_size
 
 
 def mlp_output(layer_sizes: List[int], activation: str = "tanh",
                dropout_keep_prob: float = 1.0) -> Tuple[OutputProjection, int]:
     """A multilayer perceptron over [state; embedding; contexts] (output_projection.py:163-188)."""
-    require_variant("mlp_output")
     return _MLP(layer_sizes, _activation_name(activation), dropout_keep_prob), layer_sizes[-1]

@@ -20,7 +20,6 @@ from neuralmonkey_b200.attention.base_attention import (Attendable, get_attentio
 from neuralmonkey_b200.attention.scaled_dot_product import attention, declare_attention
 from neuralmonkey_b200.attention.transformer_cross_layer import (declare_cross, flat, hierarchical,
                                                                 parallel, serial)
-from neuralmonkey_b200.nn.variants import require_variant
 from neuralmonkey_b200.decoders.autoregressive import (AutoregressiveDecoder, DecoderFeedables,
                                                        LoopState)
 from neuralmonkey_b200.decorators import tensor
@@ -98,7 +97,6 @@ class TransformerDecoder(AutoregressiveDecoder):
             raise ValueError("For the flat attention combination strategy, only a single value is "
                              "permitted in n_heads_enc.")
         if self.attention_combination_strategy in ("flat", "hierarchical"):
-            require_variant("attention_combination_strategy='{}'".format(self.attention_combination_strategy))
             self.use_kv_cache = False      # these strategies decode by re-running the prefix
         self._default_initializer = variance_scaling_initializer(mode="fan_avg", distribution="uniform")
 

@@ -17,7 +17,7 @@ from neuralmonkey_b200.model.parameterized import InitializerSpecs
 from neuralmonkey_b200.model.sequence import EmbeddedFactorSequence, EmbeddedSequence
 from neuralmonkey_b200.model.stateful import TemporalStateful, TemporalStatefulWithOutput
 from neuralmonkey_b200.nn.utils import dropout
-from neuralmonkey_b200.nn.variants import LSTMCell, NematusGRUCell, require_variant
+from neuralmonkey_b200.nn.variants import LSTMCell, NematusGRUCell
 from neuralmonkey_b200.typecheck import check_argument_types
 from neuralmonkey_b200.params import (constant_initializer, ones_initializer,
                                       orthogonal_initializer, zeros_initializer)
@@ -78,9 +78,6 @@ class RecurrentEncoder(ModelPart, TemporalStatefulWithOutput):
         if add_residual and len(set(layer_sizes)) > 1:
             raise ValueError("When using residual connectiong, all layers must have the same "
                              "size, but are {}.".format(layer_sizes))
-        for spec in self.rnn_specs:
-            if spec.cell_type != "GRU":
-                require_variant("RecurrentEncoder with rnn_cell='{}'".format(spec.cell_type))
         self._layer_sizes = layer_sizes
 
     def _cell_scopes(self, i: int, spec: RNNSpec) -> List[str]:

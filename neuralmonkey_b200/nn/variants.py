@@ -1,29 +1,18 @@
 """Model variants next to the hot path (SURVEY.md 8(f) N4): the Nematus GRU cell
-(reference: neuralmonkey/nn/ortho_gru_cell.py:57-105) and the switch that guards every variant.
+(reference: neuralmonkey/nn/ortho_gru_cell.py:57-105) and the LSTM cell.
 
 These variants are COMPOSED from operations whose kernels are parity-tested on the GPU (`ops.linear`,
 `ops.gru_layer` with one step, `ops.bahdanau_attention`) plus ONE fused kernel per step for the gate
 arithmetic (`ops.nematus_gru_gate`, `ops.lstm_gate`: nm_nematus_gate_*, nm_lstm_gate_*); they step through time instead of running the fused sequence kernels.  The oracle restates
 them and is pinned to the reference's own code (tests/test_oracle_vs_reference_code.py);
-tests/test_gpu_variants.py runs every one of them on the GPU against the oracle (round 2: all green on the
-exact engine at 1e-3 / 5e-5), so the `NMB200_UNVERIFIED` switch of round 1 is gone - `require_variant`
-remains as the (now empty) hook the constructors call."""
-import os
+tests/test_gpu_variants.py runs every one of them on the GPU against the oracle (on the exact engine at
+1e-3 / 5e-5)."""
 from typing import Tuple
 
 import torch
 
 from neuralmonkey_b200 import ops
 from neuralmonkey_b200.params import block_orthogonal_initializer, zeros_initializer
-
-
-def variants_enabled() -> bool:
-    return True
-
-
-def require_variant(what: str) -> None:
-    """Round 1 refused the variants unless NMB200_UNVERIFIED=1 was set; they are GPU-verified now."""
-    del what
 
 
 class NematusGRUCell:

@@ -7,7 +7,6 @@ may carry an ``nm_grad`` attribute (a view into the flat gradient arena of
 weight gradients straight into that arena (GEMM epilogue ``beta = 1``) and return
 ``None`` to autograd, so no torch kernels run on the weight-gradient path.
 """
-import os
 from typing import Optional, Tuple
 
 import torch
@@ -22,8 +21,6 @@ def set_gemm_backend(name: str) -> None:
     """'auto' (wgmma tensor cores when TMA-addressable), 'simt' (exact fp32) or 'tc'."""
     global _GEMM_BACKEND
     _GEMM_BACKEND = {"auto": lib.GEMM_AUTO, "simt": lib.GEMM_SIMT, "tc": lib.GEMM_TC}[name]
-    # the GRU recurrence follows: exact fp32 engine with 'simt', tensor cores otherwise
-    call("nm_gru_set_mode", 1 if name == "simt" else 0)
 
 
 def gemm_backend() -> int:
@@ -120,20 +117,16 @@ def _sink(t: torch.Tensor) -> Optional[torch.Tensor]:
 # layers and of the vocabulary projection are issued on a second stream: they fill the SMs the chain leaves idle
 # (launch latencies, short grids, the 120-CTA recurrences) instead of lengthening it.  Both streams only ever ADD
 # into disjoint parts of the flat gradient buffer: a variable's contributions all travel on the same stream.
-# Inside a CUDA-graph capture the fork and the join become graph edges.  Off unless a trainer opens the window
-# (NMB200_WGRAD_STREAM=0 keeps it shut).
+# Inside a CUDA-graph capture the fork and the join become graph edges.  Off unless a trainer opens the window.
 _wg = {"stream": None, "keep": [], "open": False}
 
 
 def weight_grad_stream(enable: bool) -> None:
-    if enable and (os.environ.get("NMB200_WGRAD_STREAM", _WGRAD_STREAM_DEFAULT) != "1" or lib.profiling()):
+    if enable and lib.profiling():
         enable = False      # (the per-call profiler times calls one by one: no overlap while it runs)
     if enable and _wg["stream"] is None:
         _wg["stream"] = torch.cuda.Stream()
     _wg["open"] = bool(enable)
-
-
-_WGRAD_STREAM_DEFAULT = "1"    # weight gradients on a second stream; NMB200_WGRAD_STREAM=0 shuts it
 
 
 def join_weight_grads() -> None:
@@ -750,13 +743,6 @@ def smoothing_term(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], 
     return _SmoothingTerm.apply(x, w, b, targets, unk_index, trans_w)
 
 
-def _xent16_enabled() -> bool:
-    """The vocabulary projection with fp16 operands and fp16 dlogits (csrc/xent16.cu) is the default on
-    the tensor-core engine; NMB200_XENT16=0 keeps every product in TF32 (the round-1 path)."""
-    import os
-    return os.environ.get("NMB200_XENT16", "1") != "0"
-
-
 def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
@@ -946,7 +932,7 @@ def logits_xent(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], tar
     """Vocabulary projection + masked cross-entropy (decoders/autoregressive.py:288-316,450-459).
 
     Returns (xent [M], lse [M], argmax [M] int64, logits [M,V] or None)."""
-    if (_xent16_enabled() and not trans_w and b is not None and _GEMM_BACKEND != lib.GEMM_SIMT
+    if (not trans_w and b is not None and _GEMM_BACKEND != lib.GEMM_SIMT
             and w.requires_grad and b.requires_grad):
         w_sink, b_sink = _sink(w), _sink(b)
         k, v = w.shape
@@ -1061,14 +1047,10 @@ class _MHATensorCore(torch.autograd.Function):
         return dq, dk, dv, None, None, None, None
 
 
-_MHA_TC_DEFAULT = "1"     # verified in tests/test_gpu_mha_tc.py; NMB200_MHA_TC=0 keeps the CUDA-core kernels
-
-
 def _mha_on_tensor_cores(bsz: int, tq: int, tk: int, heads: int, dh: int) -> bool:
     """Tensor-core attention follows the GEMM backend ('simt' = the exact fp32 kernels everywhere); whole
-    sequences only - the single-query steps of the decoding loops stay on the row kernels.  NMB200_MHA_TC=0
-    switches it off."""
-    if _GEMM_BACKEND == lib.GEMM_SIMT or os.environ.get("NMB200_MHA_TC", _MHA_TC_DEFAULT) == "0" or tq < 8:
+    sequences only - the single-query steps of the decoding loops stay on the row kernels."""
+    if _GEMM_BACKEND == lib.GEMM_SIMT or tq < 8:
         return False
     return bool(lib.load().nm_mha_tc_supported(bsz, tq, tk, heads, dh))
 

@@ -163,73 +163,39 @@ class GenericTrainer(GraphExecutor, Feedable):
             t.register_hook(hook)
         works.append(("armed", fired, early))
 
-    @staticmethod
-    def _update_in_ranges() -> bool:
-        """NMB200_RANGE_UPDATE=1: optimizer range by range behind the exchange (see `_finish_exchange`).  Off by
-        default: on two GPUs it takes the en-de step from 6.63 to 6.43 ms, but on four and eight GPUs the
-        graph-replayed loop then spends 4-6 ms of HOST time per step inside the graph launch (device-resident
-        loop slower than the end-to-end one) - measured with the round's last GPU minutes and not understood
-        yet; the default is the path whose eight-GPU run was clean (DESIGN.md section 6)."""
-        import os
-        return os.environ.get("NMB200_RANGE_UPDATE", "0") == "1"
-
-    def _finish_exchange(self, works: list, update=None) -> bool:
+    def _finish_exchange(self, works: list) -> None:
         """All-reduce what the hook did not cover (the encoders' ranges and the statistic slots - or, when
-        it never fired, everything) and make the compute stream wait for the exchange.
-
-        With `update` (a callable taking a list of (lo, hi) ranges of the flat buffer) and an early exchange
-        under way, the optimizer runs RANGE BY RANGE: the decoder-side ranges are updated as soon as their
-        all-reduce is back - while the encoder ranges are still travelling - and the encoder ranges after
-        theirs.  The global token count the update divides by was all-reduced on its own at the start of the
-        backward pass (`_count_global`).  Returns True when `update` did the optimizer's work."""
+        it never fired, everything) and make the compute stream wait for the exchange."""
         arena = runtime.arena()
-        _enc, early, late = self._exchange_plan()
+        _enc, _early, late = self._exchange_plan()
         armed = [w for w in works if isinstance(w, tuple) and w[0] == "armed"]
-        done_early = bool(armed and armed[0][1])
-        counted = [w for w in works if isinstance(w, tuple) and w[0] == "count"]
-        early_handles = [w for w in works if not isinstance(w, tuple)]
-        late_handles = []
+        handles = [w for w in works if not isinstance(w, tuple)]
         tail = arena.trainable_size
-        if done_early:
+        if armed and armed[0][1]:
             ranges = list(late)
             if ranges and ranges[-1][1] == tail:
                 ranges[-1] = (ranges[-1][0], tail + arena.STAT_SLOTS)        # stats ride with the last range
             else:
                 ranges.append((tail, tail + arena.STAT_SLOTS))
             for lo, hi in ranges:
-                late_handles.append(distributed.all_reduce_async(arena.grad_buffer[lo:hi]))
+                handles.append(distributed.all_reduce_async(arena.grad_buffer[lo:hi]))
         else:
-            late_handles.append(distributed.all_reduce_async(arena.allreduce_view))
+            handles.append(distributed.all_reduce_async(arena.allreduce_view))
         timed = arena.params.is_cuda and not torch.cuda.is_current_stream_capturing()
-        waits = []
-
-        def wait_for(handles):
-            if timed:
-                ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                ev0.record()
-            for h in handles:
-                if h is not None:
-                    h.wait()
-            if timed:
-                ev1.record()
-                waits.append((ev0, ev1))
-
-        in_ranges = bool(update is not None and done_early and counted)
-        if in_ranges:
-            wait_for([counted[0][1]] + early_handles)
-            update(list(early))
-            wait_for(late_handles)
-            update(list(late))
-        else:
-            wait_for([w[1] for w in counted] + early_handles + late_handles)
+        if timed:
+            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev0.record()
+        for h in handles:
+            if h is not None:
+                h.wait()
         if timed:       # how long the compute stream waited for the exchange after the backward pass was issued
+            ev1.record()
             history = getattr(self, "_comm_history", None)
             if history is None:
                 history = self._comm_history = []
-            history.append(waits)
+            history.append([(ev0, ev1)])
             del history[:-8]
         del works[:]
-        return in_ranges
 
     # -- one optimisation step ---------------------------------------------------------------
     def _backward(self, works: Optional[list] = None) -> Dict[str, torch.Tensor]:
@@ -247,13 +213,6 @@ class GenericTrainer(GraphExecutor, Feedable):
             # optimizer kernel -> N ranks reproduce the single-GPU token mean exactly
             loss_sum, count = exact
             w = self.objectives[0].weight
-            if works is not None and self._update_in_ranges():
-                # the token count is known before the backward pass: exchanged on its own, right away, so that
-                # the optimizer can start on the ranges that come back first
-                if getattr(self, "_count_global", None) is None:
-                    self._count_global = torch.zeros(1, device=arena.params.device, dtype=torch.float32)
-                self._count_global.copy_(count.detach().reshape(1))
-                works.append(("count", distributed.all_reduce_async(self._count_global)))
             ops.weight_grad_stream(arena.params.is_cuda)
             try:
                 (loss_sum if w is None else loss_sum * w).backward()
@@ -318,9 +277,8 @@ class GenericTrainer(GraphExecutor, Feedable):
                         arena.zero_grad()
                         works = []
                         self._backward(works)
-                        if not self._finish_exchange(works, lambda ranges: self._adam_kernel(
-                                1.0, self._count_global, 0.0, self._lr_dev, ranges=ranges)):
-                            self._adam_kernel(1.0, arena.stats[1:2], 0.0, self._lr_dev)
+                        self._finish_exchange(works)
+                        self._adam_kernel(1.0, arena.stats[1:2], 0.0, self._lr_dev)
                 elif distributed.world_size() > 1:
                     # the gradient exchange stays an eager NCCL call between two captured halves
                     # (backward | clip + Adam)
@@ -386,9 +344,7 @@ class GenericTrainer(GraphExecutor, Feedable):
             if world > 1:
                 if info["exact"] and grad_scale == 1.0:
                     lr_t = self._advance_step()
-                    if self._finish_exchange(works, lambda ranges: self._adam_kernel(
-                            1.0, self._count_global, lr_t, None, ranges=ranges)):
-                        return {"losses": [arena.stats[0] / arena.stats[1]], "l1l2": self._l1l2}
+                    self._finish_exchange(works)
                     self._adam_kernel(1.0, arena.stats[1:2], lr_t, None)
                     return {"losses": [arena.stats[0] / arena.stats[1]], "l1l2": self._l1l2}
                 self._finish_exchange(works)
@@ -441,31 +397,9 @@ class GenericTrainer(GraphExecutor, Feedable):
                         denominator: Optional[torch.Tensor] = None) -> None:
         self._adam_kernel(grad_scale, denominator, self._advance_step(), None)
 
-    def _segments_of(self, ranges):
-        """(first segment, number of segments, offsets relative to the range's first float) per (lo, hi) range of the
-        flat buffer; ranges are unions of whole variables (`_exchange_plan`).  Built once (the layout never
-        changes), with the plan - i.e. in an eagerly issued step, never inside a graph capture."""
-        cache = getattr(self, "_range_tables", None)
-        if cache is None:
-            cache = self._range_tables = {}
-        arena = runtime.arena()
-        out = []
-        for lo, hi in ranges:
-            if (lo, hi) not in cache:
-                offs = [int(o) for o in arena.seg_off.tolist()]
-                first, last = offs.index(lo), offs.index(hi)
-                rel = torch.tensor([o - lo for o in offs[first:last + 1]], dtype=torch.int64,
-                                   device=arena.seg_off.device)
-                cache[(lo, hi)] = (first, last - first, rel)
-            out.append(cache[(lo, hi)])
-        return out
-
     def _adam_kernel(self, grad_scale: float, denominator: Optional[torch.Tensor], lr_t: float,
-                     lr_t_dev: Optional[torch.Tensor], ranges=None) -> None:
-        """Clip + regularise + Adam over the whole flat buffer, or (`ranges`: (lo, hi) float ranges made of whole
-        variables) over those ranges only - the L1 / L2 sums the trainer reports then accumulate over the calls
-        of a step, the first of which (the call whose first range starts the exchange plan's early list, or any
-        whole-buffer call) resets them."""
+                     lr_t_dev: Optional[torch.Tensor]) -> None:
+        """Clip + regularise + Adam over the whole flat buffer."""
         arena = runtime.arena()
         opt = self.optimizer
         if not hasattr(self, "_l1l2_buf"):
@@ -485,26 +419,10 @@ class GenericTrainer(GraphExecutor, Feedable):
             arena.grads.mul_(mask)
         common = (float(opt.beta1), float(opt.beta2), float(opt.epsilon),
                   float(self.clip_norm) if self.clip_norm else 0.0, float(self.l1_weight), float(self.l2_weight))
-        if ranges is None:
-            call("nm_clip_adam_step", ptr(arena.params), ptr(arena.grads), ptr(adam_m),
-                 ptr(adam_v), ptr(arena.seg_off), ptr(seg_flags), ptr(arena.seg_norms), n,
-                 len(arena.train_names), float(grad_scale), ptr(denominator), float(lr_t), *common,
-                 ptr(self._l1l2_buf), ptr(lr_t_dev), lib.stream())
-            return
-        if not hasattr(self, "_l1l2_part"):
-            self._l1l2_part = torch.zeros(2, device=arena.params.device, dtype=torch.float32)
-        _enc, early, _late = self._exchange_plan()
-        for (first, count, rel), (lo, hi) in zip(self._segments_of(ranges), ranges):
-            if count <= 0:
-                continue
-            call("nm_clip_adam_step", ptr(arena.params[lo:]), ptr(arena.grads[lo:]), ptr(adam_m[lo:]),
-                 ptr(adam_v[lo:]), ptr(rel), ptr(seg_flags[first:]), ptr(arena.seg_norms[first:]), hi - lo,
-                 count, float(grad_scale), ptr(denominator), float(lr_t), *common,
-                 ptr(self._l1l2_part), ptr(lr_t_dev), lib.stream())
-            if early and lo == early[0][0]:
-                self._l1l2_buf.copy_(self._l1l2_part)       # first range of the step
-            else:
-                self._l1l2_buf.add_(self._l1l2_part)
+        call("nm_clip_adam_step", ptr(arena.params), ptr(arena.grads), ptr(adam_m),
+             ptr(adam_v), ptr(arena.seg_off), ptr(seg_flags), ptr(arena.seg_norms), n,
+             len(arena.train_names), float(grad_scale), ptr(denominator), float(lr_t), *common,
+             ptr(self._l1l2_buf), ptr(lr_t_dev), lib.stream())
 
     @property
     def _l1l2(self) -> torch.Tensor:

@@ -134,12 +134,10 @@ def xent_rows(logits, targets=None, weights=None, want_argmax=False, first_col=0
     return lse, xent, (torch.argmax(part, dim=-1) if want_argmax else None)
 
 
-def adam_kernel(trainer, grad_scale, denominator, lr_t, lr_t_dev, ranges=None):
+def adam_kernel(trainer, grad_scale, denominator, lr_t, lr_t_dev):
     """Stand-in for GenericTrainer._adam_kernel (`nm_clip_adam_step`) over the arena's gradient buffer
     (the stand-in ops leave their gradients in `.grad`; the trainer folds those in).  Same order as the
-    kernel: scale, add the L1 / L2 terms of the regularised variables, clip per tensor, TF-Adam.  `ranges`
-    ((lo, hi) float ranges of the flat buffer): only the variables inside them, the L1 / L2 sums accumulating
-    over the calls of a step as in the trainer."""
+    kernel: scale, add the L1 / L2 terms of the regularised variables, clip per tensor, TF-Adam."""
     from neuralmonkey_b200 import runtime
     arena, opt = runtime.arena(), trainer.optimizer
     scale = float(grad_scale) / (float(denominator) if denominator is not None else 1.0)
@@ -149,8 +147,6 @@ def adam_kernel(trainer, grad_scale, denominator, lr_t, lr_t_dev, ranges=None):
     l1 = l2 = 0.0
     with torch.no_grad():
         for name in trainer.var_list:                 # with var_scopes: only the variables in scope
-            if ranges is not None and not any(lo <= arena.variables[name].offset < hi for lo, hi in ranges):
-                continue
             var = arena.get(name)
             grad = arena.grad(name) * scale           # the trainer folded the autograd gradients in
             if O.is_regularizable(name):
@@ -165,12 +161,7 @@ def adam_kernel(trainer, grad_scale, denominator, lr_t, lr_t_dev, ranges=None):
             m.mul_(opt.beta1).add_(grad, alpha=1 - opt.beta1)
             v.mul_(opt.beta2).addcmul_(grad, grad, value=1 - opt.beta2)
             var.sub_((float(lr_t_dev) if lr_t_dev is not None else lr_t) * m / (v.sqrt() + opt.epsilon))
-    first_of_step = ranges is None or (trainer._exchange_plan()[1] and ranges[0][0] == trainer._exchange_plan()[1][0][0])
-    if first_of_step:
-        trainer._l1l2_buf[0], trainer._l1l2_buf[1] = l1, l2
-    else:
-        trainer._l1l2_buf[0] += l1
-        trainer._l1l2_buf[1] += l2
+    trainer._l1l2_buf[0], trainer._l1l2_buf[1] = l1, l2
 
 
 def nematus_gru_gate(state_gates, input_gates, state_cand, input_cand, state):

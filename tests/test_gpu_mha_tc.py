@@ -36,9 +36,8 @@ def _reference(q, k, v, mask, causal, heads, drop):
 @pytest.mark.parametrize("causal", [False, True])
 @pytest.mark.parametrize("use_mask", [False, True])
 @pytest.mark.parametrize("shape", SHAPES)
-def test_tensor_core_attention(monkeypatch, shape, use_mask, causal, use_drop):
+def test_tensor_core_attention(shape, use_mask, causal, use_drop):
     from neuralmonkey_b200 import lib, ops
-    monkeypatch.setenv("NMB200_MHA_TC", "1")
     bsz, tq, tk, heads, dh = shape
     if causal:
         tk = tq
@@ -83,11 +82,10 @@ def test_tensor_core_attention(monkeypatch, shape, use_mask, causal, use_drop):
     assert abs(float(tc[1].sum(-1).mean()) - 1.0) < 1e-4
 
 
-def test_padding_of_the_weight_matrices_is_zero(monkeypatch):
+def test_padding_of_the_weight_matrices_is_zero():
     """The [Tq32, Tk32] storage behind the returned weights: the padding must be zeros (the backward products
     reduce over whole 32-element blocks of it)."""
     from neuralmonkey_b200 import ops
-    monkeypatch.setenv("NMB200_MHA_TC", "1")
     g = torch.Generator().manual_seed(1)
     q, k, v = (torch.randn(2, t, 64, generator=g).cuda() for t in (37, 50, 50))
     _out, weights = ops.mha_core(q, k, v, None, False, 2)

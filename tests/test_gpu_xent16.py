@@ -1,5 +1,5 @@
 """The fp16-operand vocabulary projection (csrc/xent16.cu, ops._LogitsXent16: the default on the
-tensor-core engine) against fp64 references and against the TF32 path (NMB200_XENT16=0)."""
+tensor-core engine) against fp64 references and against the TF32 path (ops._LogitsXent)."""
 import pytest
 import torch
 
@@ -91,7 +91,7 @@ def test_gemm_f16_tn(m, n, k, beta):
 
 
 @pytest.mark.parametrize("m,k,v,unk", [(96, 24, 200, 3), (1100, 300, 4100, -1)])
-def test_logits_xent16_matches_the_default_path(monkeypatch, m, k, v, unk):
+def test_logits_xent16_matches_the_tf32_path(m, k, v, unk):
     from neuralmonkey_b200 import ops
     g = torch.Generator().manual_seed(2)
     x0 = (torch.randn(m, k, generator=g) * 0.7).cuda()
@@ -105,12 +105,14 @@ def test_logits_xent16_matches_the_default_path(monkeypatch, m, k, v, unk):
     weights = (torch.rand(m, generator=g) > 0.2).float().cuda()
     results = {}
     for mode in ("0", "1"):
-        monkeypatch.setenv("NMB200_XENT16", mode)
         grads.zero_()
         x = x0.clone().requires_grad_(True)
         wv, bv = w.detach().requires_grad_(True), b.detach().requires_grad_(True)
         wv.nm_grad, bv.nm_grad = grads[:k * v].view(k, v), grads[k * v:]
-        xent, lse, argmax, logits = ops.logits_xent(x, wv, bv, targets, weights, unk, False, keep_logits=True)
+        if mode == "0":     # every product in TF32
+            xent, lse, argmax, logits = ops._LogitsXent.apply(x, wv, bv, targets, weights, unk, False, True)
+        else:               # ops.logits_xent's choice for these inputs: fp16 operands
+            xent, lse, argmax, logits = ops.logits_xent(x, wv, bv, targets, weights, unk, False, keep_logits=True)
         (xent.sum() / weights.sum()).backward()
         results[mode] = (xent.detach().clone(), lse.clone(), argmax.clone(), logits.clone(), x.grad.clone(),
                          grads.clone())

@@ -366,10 +366,6 @@ def test_weight_gradient_window_stays_shut_without_a_gpu_and_while_profiling(mon
     ops._off_the_chain(lambda: ran.append(1))        # window shut: runs in place, keeps nothing alive
     assert ran == [1] and not ops._wg["keep"]
     ops.join_weight_grads()                           # nothing to wait for
-    monkeypatch.setenv("NMB200_WGRAD_STREAM", "0")
-    ops.weight_grad_stream(True)
-    assert ops._wg["open"] is False
-    monkeypatch.setenv("NMB200_WGRAD_STREAM", "1")
     monkeypatch.setattr(lib, "_profile", {})          # as between profile_start() and profile_stop()
     ops.weight_grad_stream(True)
     assert ops._wg["open"] is False

@@ -22,7 +22,6 @@ def cpu_model(monkeypatch):
     for name in cpu_ops.STAND_INS:
         monkeypatch.setattr(ops, name, getattr(cpu_ops, name))
     monkeypatch.setattr(runtime, "_device", torch.device("cpu"))
-    monkeypatch.setenv("NMB200_UNVERIFIED", "1")
     yield
     runtime.reset()
 
@@ -263,10 +262,9 @@ def test_decoder_and_encoder_variants(cpu_model, cell, conditional, out_proj, en
     assert max_abs(out.last_search_step_output.scores, want["scores"]) < 1e-4
 
 
-def test_variants_need_no_switch_any_more(cpu_model, monkeypatch):
-    """Round 1 kept the N4 variants behind NMB200_UNVERIFIED=1 until they had run on a GPU; they have
-    (tests/test_gpu_variants.py), so they build without it."""
-    monkeypatch.delenv("NMB200_UNVERIFIED", raising=False)
+def test_variant_configurations_build(cpu_model):
+    """A decoder with Nematus GRU cells, the conditional GRU and a maxout output, and a GRU decoder with the
+    Nematus output projection, build like any other configuration."""
     assert _build_variant("NematusGRU", True, "maxout", "linear", "GRU") is not None
     assert _build_variant("GRU", False, "nematus", "linear", "GRU") is not None
 

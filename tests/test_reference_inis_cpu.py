@@ -42,7 +42,6 @@ def test_reference_ini_trains_unchanged(monkeypatch, tmp_path, name):
         monkeypatch.setattr(ops, op, getattr(cpu_ops, op))
     monkeypatch.setattr(runtime, "_device", torch.device("cpu"))
     monkeypatch.setattr(GenericTrainer, "_adam_kernel", cpu_ops.adam_kernel)
-    monkeypatch.setenv("NMB200_UNVERIFIED", "1")          # small.ini: Nematus GRU cells, conditional GRU
     monkeypatch.setenv("NEURALMONKEY_STRICT", "1")        # as tests_run.sh: warnings are errors
     monkeypatch.setenv("NM_EXPERIMENT_NAME", "small")     # small.ini reads it from the environment
     unpack(str(tmp_path / "tree"))
