@@ -218,11 +218,12 @@ int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask,
 /* ---- K5/K6: vocabulary projection loss ---------------------------------------
  * Replaces log_softmax + tf.contrib.seq2seq.sequence_loss
  * (decoders/autoregressive.py:288-316) and the greedy argmax (:446-480).
- * logits [M,V] (already includes bias and the -1e9 <unk> mask).
+ * logits [M,V] (already includes the bias).  unk_index >= 0: -1e9 is added to
+ * column unk_index of every row and written back to logits (the <unk> mask).
  * Per row m: lse[m] = logsumexp_v logits; xent[m] = (lse - logits[m,target[m]])
  * * weight[m]; argmax[m] = first index of the row maximum (tf.argmax order).
  * targets may be NULL (then xent is not written). */
-int nm_xent_fwd(const float* logits, const int64_t* targets, const float* weights,
+int nm_xent_fwd(float* logits, int64_t unk_index, const int64_t* targets, const float* weights,
                 float* lse, float* xent, int64_t* argmax, int64_t M, int64_t V,
                 int64_t ldl, void* stream);
 /* dlogits[m,v] = (exp(logits[m,v]-lse[m]) - [v==target[m]]) * weights[m] * scale[0]

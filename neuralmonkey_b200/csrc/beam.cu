@@ -338,6 +338,23 @@ __global__ void beam_gather_kernel(const uint8_t* __restrict__ x, const int32_t*
   }
 }
 
+// token_ids[t, b, j] of the hypotheses that survive: walk the (word, parent) records backwards
+// (what re-gathering the whole token history at every step computes, beam_search_decoder.py:546-551).
+__global__ void beam_backtrack_kernel(const int64_t* __restrict__ first, const int64_t* __restrict__ words,
+                                      const int32_t* __restrict__ parents, int64_t* __restrict__ out,
+                                      int64_t rows, int64_t k, int64_t steps) {
+  const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // b*k + j
+  if (o >= rows) return;
+  const int64_t b = o / k;
+  int64_t cur = o - b * k;
+  for (int64_t t = steps; t >= 1; --t) {
+    const int64_t src = (t - 1) * rows + b * k + cur;
+    out[t * rows + o] = words[src];
+    cur = parents[src];
+  }
+  out[o] = first[b * k + cur];
+}
+
 }  // namespace nm
 
 using namespace nm;
@@ -409,6 +426,18 @@ int nm_beam_gather(const void* x, const int32_t* beam_ids, void* out, int64_t B,
                                                              beam_ids, reinterpret_cast<uint8_t*>(out),
                                                              k, row_bytes);
   NM_LAUNCH_CHECK("nm_beam_gather");
+  return NM_OK;
+}
+
+int nm_beam_backtrack(const int64_t* first_symbols, const int64_t* words, const int32_t* parents,
+                      int64_t* token_ids, int64_t B, int64_t k, int64_t steps, void* stream) {
+  NM_REQUIRE(first_symbols && token_ids && B > 0 && k > 0 && steps >= 0, NM_E_INVALID,
+             "nm_beam_backtrack: bad arguments");
+  NM_REQUIRE(steps == 0 || (words && parents), NM_E_INVALID, "nm_beam_backtrack: null step records");
+  const int64_t rows = B * k;
+  beam_backtrack_kernel<<<(unsigned)ceil_div(rows, 128), 128, 0, (cudaStream_t)stream>>>(
+      first_symbols, words, parents, token_ids, rows, k, steps);
+  NM_LAUNCH_CHECK("nm_beam_backtrack");
   return NM_OK;
 }
 

@@ -1,6 +1,5 @@
 // HBM-bound kernels of the hot path: embedding gather/scatter (K1), activation
-// backward, bias-gradient column sums, maxout, layer norm (K7), and the
-// row-wise softmax-cross-entropy statistics over materialised logits (K5/K6).
+// backward, bias-gradient column sums, maxout and layer norm (K7).
 // All are grid-stride / one-warp-per-row kernels with 16-byte vector accesses
 // where the row length allows it.
 #include "common.cuh"
@@ -282,95 +281,6 @@ __global__ void layernorm_bwd_param_kernel(const float* __restrict__ x, const fl
   }
 }
 
-// ---------------------------------------------------------------------------
-// K5/K6 on materialised logits: one block per row.
-// ---------------------------------------------------------------------------
-struct MaxIdx {
-  float v;
-  int64_t i;
-};
-__device__ __forceinline__ MaxIdx better(MaxIdx a, MaxIdx b) {
-  // larger value wins; ties go to the lower index (tf.argmax / np.argmax order)
-  if (b.v > a.v || (b.v == a.v && b.i < a.i)) return b;
-  return a;
-}
-__device__ __forceinline__ MaxIdx warp_best(MaxIdx a) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    MaxIdx b;
-    b.v = __shfl_xor_sync(0xffffffffu, a.v, o);
-    b.i = __shfl_xor_sync(0xffffffffu, a.i, o);
-    a = better(a, b);
-  }
-  return a;
-}
-
-__global__ void xent_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ targets,
-                                const float* __restrict__ weights, float* __restrict__ lse,
-                                float* __restrict__ xent, int64_t* __restrict__ argmax, int64_t V,
-                                int64_t ldl) {
-  __shared__ float red[32];
-  __shared__ float sv[32];
-  __shared__ int64_t si[32];
-  const int64_t row = blockIdx.x;
-  const float* lr = logits + row * ldl;
-  MaxIdx best{-INFINITY, (int64_t)0x7fffffffffffffffLL};
-  for (int64_t c = threadIdx.x; c < V; c += blockDim.x) {
-    const float x = lr[c];
-    if (x > best.v) { best.v = x; best.i = c; }
-  }
-  best = warp_best(best);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (lane == 0) { sv[w] = best.v; si[w] = best.i; }
-  __syncthreads();
-  if (w == 0) {
-    const int nw = blockDim.x >> 5;
-    MaxIdx b{lane < nw ? sv[lane] : -INFINITY, lane < nw ? si[lane] : (int64_t)0x7fffffffffffffffLL};
-    b = warp_best(b);
-    if (lane == 0) { sv[0] = b.v; si[0] = b.i; }
-  }
-  __syncthreads();
-  const float mx = sv[0];
-  float s = 0.f;
-  for (int64_t c = threadIdx.x; c < V; c += blockDim.x) s += expf(lr[c] - mx);
-  s = block_sum(s, red);
-  if (threadIdx.x == 0) {
-    const float l = mx + logf(s);
-    lse[row] = l;
-    if (argmax) argmax[row] = si[0];
-    if (targets && xent) {
-      const float wgt = weights ? weights[row] : 1.f;
-      xent[row] = (l - lr[targets[row]]) * wgt;
-    }
-  }
-}
-
-__global__ void xent_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ targets,
-                                const float* __restrict__ weights, const float* __restrict__ lse,
-                                const float* __restrict__ scale, float* __restrict__ dlogits,
-                                int64_t V, int64_t ldl) {
-  const int64_t row = blockIdx.y;
-  const float wgt = (weights ? weights[row] : 1.f) * scale[0];
-  const float l = lse[row];
-  const int64_t tgt = targets[row];
-  const float* lr = logits + row * ldl;
-  float* dr = dlogits + row * ldl;
-  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < V;
-       c += (int64_t)gridDim.x * blockDim.x) {
-    const float p = expf(lr[c] - l);
-    dr[c] = (p - (c == tgt ? 1.f : 0.f)) * wgt;
-  }
-}
-
-__global__ void log_softmax_kernel(const float* __restrict__ logits, const float* __restrict__ lse,
-                                   float* __restrict__ out, int64_t V, int64_t ldl) {
-  const int64_t row = blockIdx.y;
-  const float l = lse[row];
-  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < V;
-       c += (int64_t)gridDim.x * blockDim.x)
-    out[row * V + c] = logits[row * ldl + c] - l;
-}
-
 static inline int grid_for(int64_t work_items, int threads, int blocks_per_sm = 8) {
   const int64_t need = ceil_div(work_items, threads);
   const int64_t cap = (int64_t)sm_count() * blocks_per_sm;
@@ -521,43 +431,6 @@ int nm_layernorm_bwd(const float* x, const float* gamma, const float* mean, cons
   layernorm_bwd_param_kernel<<<grid, block, 0, s>>>(x, mean, rstd, dy, dgamma, dbeta, M, (int)D,
                                                     (int)rows_per_block);
   NM_LAUNCH_CHECK("nm_layernorm_bwd(param)");
-  return NM_OK;
-}
-
-int nm_xent_fwd(const float* logits, const int64_t* targets, const float* weights, float* lse,
-                float* xent, int64_t* argmax, int64_t M, int64_t V, int64_t ldl, void* stream) {
-  NM_REQUIRE(logits && lse, NM_E_INVALID, "nm_xent_fwd: null pointer");
-  NM_REQUIRE(M >= 0 && V > 0 && ldl >= V, NM_E_INVALID, "nm_xent_fwd: bad sizes");
-  if (M == 0) return NM_OK;
-  const int threads = V >= 4096 ? 512 : (V >= 256 ? 128 : 32);
-  xent_fwd_kernel<<<(unsigned)M, threads, 0, (cudaStream_t)stream>>>(logits, targets, weights, lse,
-                                                                     xent, argmax, V, ldl);
-  NM_LAUNCH_CHECK("nm_xent_fwd");
-  return NM_OK;
-}
-
-int nm_xent_bwd(const float* logits, const int64_t* targets, const float* weights, const float* lse,
-                const float* scale, float* dlogits, int64_t M, int64_t V, int64_t ldl, void* stream) {
-  NM_REQUIRE(logits && targets && lse && scale && dlogits, NM_E_INVALID, "nm_xent_bwd: null pointer");
-  NM_REQUIRE(M >= 0 && V > 0 && ldl >= V, NM_E_INVALID, "nm_xent_bwd: bad sizes");
-  NM_REQUIRE(M <= 65535, NM_E_UNSUPPORTED, "nm_xent_bwd: M > 65535 rows per call");
-  if (M == 0) return NM_OK;
-  dim3 grid((unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64), (unsigned)M);
-  xent_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, targets, weights, lse, scale,
-                                                          dlogits, V, ldl);
-  NM_LAUNCH_CHECK("nm_xent_bwd");
-  return NM_OK;
-}
-
-int nm_log_softmax(const float* logits, const float* lse, float* logprobs, int64_t M, int64_t V,
-                   int64_t ldl, void* stream) {
-  NM_REQUIRE(logits && lse && logprobs, NM_E_INVALID, "nm_log_softmax: null pointer");
-  NM_REQUIRE(M >= 0 && V > 0 && ldl >= V, NM_E_INVALID, "nm_log_softmax: bad sizes");
-  NM_REQUIRE(M <= 65535, NM_E_UNSUPPORTED, "nm_log_softmax: M > 65535 rows per call");
-  if (M == 0) return NM_OK;
-  dim3 grid((unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64), (unsigned)M);
-  log_softmax_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, lse, logprobs, V, ldl);
-  NM_LAUNCH_CHECK("nm_log_softmax");
   return NM_OK;
 }
 

@@ -1,6 +1,6 @@
 // The vocabulary projection with fp16 operands (K5/K6), the default of ops.logits_xent on the tensor-core engine
 // (ops._LogitsXent16; tied embeddings, the exact engine and weights without gradient-buffer sinks keep every
-// product in TF32, xent_tc.cu).
+// product in TF32, xent.cu).
 //
 // The three kernels that touch dlogits [M,V] are a large part of a training step; in fp32 the matrix is
 // written once (1.6 GB at the bench shape) and read about three times.  Here it is stored once as fp16,

@@ -156,14 +156,13 @@ class RNNDecodeEngine:
              ptr(sym_out), ptr(fin_out), ptr(mask_out), ptr(count), ptr(part), ptr(logits), d["V"], rows,
              d["V"], d["O"], ops.gemm_backend(), lib.stream())
 
-    def _tc_logits(self, rows: int, d: Dict[str, int]) -> bool:
-        """Whether the vocabulary projection of a step runs on the tensor cores (else: exact fp32 CUDA
-        cores into a materialised [rows, V] buffer)."""
+    def _tc_logits(self, x: torch.Tensor, d: Dict[str, int]) -> bool:
+        """Whether the vocabulary projection of a step over `x` [rows, O] runs on the tensor cores (else: exact
+        fp32 CUDA cores into a materialised [rows, V] buffer)."""
         dec = self.dec
         wmat = dec.decoding_w
-        return (ops.gemm_backend() != lib.GEMM_SIMT and
-                lib.load().nm_gemm_uses_tc(0, int(dec._w_transposed), rows, d["V"], d["O"], d["O"],
-                                           wmat.stride(0), d["V"]) == 1 and wmat.data_ptr() % 16 == 0)
+        return ops._on_tensor_cores(False, dec._w_transposed, x.size(0), d["V"], d["O"], x, x.stride(0), wmat,
+                                    wmat.stride(0), ops.gemm_backend())
 
     def _run_chunks(self, key, kind: str, steps: int, first_step: int, step_fn, counts: torch.Tensor) -> int:
         """Issue steps first_step..steps-1 in chunks; returns how many steps the reference loop runs:
@@ -218,7 +217,7 @@ class RNNDecodeEngine:
             gsteps = min(int(gold.shape[0]), max_steps)
             b["gold"][:gsteps].copy_(gold[:gsteps])
             b["goldw"][:gsteps].copy_(gold_mask[:gsteps].to(torch.float32))
-        use_tc = self._tc_logits(rows, d)
+        use_tc = self._tc_logits(b["out"][0], d)      # step t reads b["out"][t], aligned as b["out"][0]
         if not use_tc and b["logits1"] is None:
             b["logits1"] = torch.zeros(rows, d["V"], device=runtime.device())
 
@@ -256,7 +255,7 @@ class RNNDecodeEngine:
         b = self._buffers(key, rows, nb, tx, max_steps, k)
         w = self._weights()
         self._load_encoder(b, k)
-        use_tc = self._tc_logits(rows, d)
+        use_tc = self._tc_logits(b["out"], d)
         b["counts"].zero_()
         b["counts"][0] = 1                    # slot 0 is the initial decoder step, not a search step
         b["fin"].zero_()

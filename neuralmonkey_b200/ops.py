@@ -846,9 +846,7 @@ class _LogitsXent(torch.autograd.Function):
         argmax = torch.empty(m, device=dev, dtype=torch.int64)
         w2, ldw = _rows(w)
         logits = torch.empty(m, v, device=dev, dtype=torch.float32) if keep_logits else None
-        fused = (_GEMM_BACKEND != lib.GEMM_SIMT and
-                 lib.load().nm_gemm_uses_tc(0, int(trans_w), m, v, k, ldx, ldw, v) == 1 and
-                 x2.data_ptr() % 16 == 0 and w2.data_ptr() % 16 == 0)
+        fused = _on_tensor_cores(False, trans_w, m, v, k, x2, ldx, w2, ldw, _GEMM_BACKEND)
         if fused:
             part = torch.empty(lib.load().nm_logits_xent_scratch(m, v), device=dev,
                                dtype=torch.float32)
@@ -858,13 +856,8 @@ class _LogitsXent(torch.autograd.Function):
         else:
             if logits is None:
                 logits = torch.empty(m, v, device=dev, dtype=torch.float32)
-            bias_eff = b
-            if unk_index >= 0:  # fold the -1e9 <unk> mask into the bias vector ([V], host plumbing)
-                bias_eff = b.detach().clone() if b is not None else torch.zeros(
-                    v, device=dev, dtype=torch.float32)
-                bias_eff[unk_index] += -1e9
-            gemm(x2, w2, logits, trans_b=trans_w, bias=bias_eff)
-            call("nm_xent_fwd", ptr(logits), ptr(targets), ptr(weights), ptr(lse), ptr(xent),
+            gemm(x2, w2, logits, trans_b=trans_w, bias=b)
+            call("nm_xent_fwd", ptr(logits), unk_index, ptr(targets), ptr(weights), ptr(lse), ptr(xent),
                  ptr(argmax), m, v, v, lib.stream())
         ctx.save_for_backward(x2, w2, b, targets, weights, lse, None if fused else logits)
         ctx.cfg = (fused, unk_index, trans_w, x.shape)
@@ -903,19 +896,6 @@ class _LogitsXent(torch.autograd.Function):
             dx = dx.view(in_shape)
         w_sink, b_sink = ctx.sinks
         want_w, want_b = ctx.needs_input_grad[1], b is not None and ctx.needs_input_grad[2]
-        if (want_w and want_b and not trans_w and w_sink is not None and b_sink is not None
-                and b_sink.data_ptr() == w_sink.data_ptr() + 4 * k * v and w_sink.is_contiguous()):
-            # The bias gradient is the column sum of dlogits = one more row of X^T . dlogits with a
-            # column of ones appended to X, and the bias segment sits right behind the weight
-            # segment in the flat gradient buffer: ONE GEMM writes both (the 301st row costs no
-            # extra tile) instead of re-reading the [M,V] matrix for a column sum.
-            kpad = (k + 1 + 3) // 4 * 4
-            x_aug = torch.zeros(m, kpad, device=dev, dtype=torch.float32)
-            x_aug[:, :k] = x2
-            x_aug[:, k] = 1.0
-            sink_aug = torch.as_strided(w_sink, (k + 1, v), (v, 1))
-            gemm(x_aug[:, :k + 1], dlogits, sink_aug, trans_a=True, beta=1.0)
-            return dx, None, None, None, None, None, None, None
         if want_w:
             if trans_w:   # w is [V,K]: dW = dlogits^T @ x
                 dw = _weight_grad(dlogits, x2, True, False, w_sink, w2.shape)
@@ -1080,7 +1060,7 @@ def xent_rows(logits: torch.Tensor, targets: Optional[torch.Tensor] = None,
     lse = torch.empty(m, device=dev, dtype=torch.float32)
     xent = torch.empty(m, device=dev, dtype=torch.float32) if targets is not None else None
     arg = torch.empty(m, device=dev, dtype=torch.int64) if want_argmax else None
-    call("nm_xent_fwd", ptr(logits) + 4 * first_col, ptr(targets), ptr(weights), ptr(lse), ptr(xent),
+    call("nm_xent_fwd", ptr(logits) + 4 * first_col, -1, ptr(targets), ptr(weights), ptr(lse), ptr(xent),
          ptr(arg), m, v - first_col, v, lib.stream())
     return lse, xent, arg
 
