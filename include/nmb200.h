@@ -58,7 +58,8 @@ int nm_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* ---- K1: embedding lookup -------------------------------------------------
  * Replaces tf.nn.embedding_lookup * mask (neuralmonkey/model/sequence.py:181-191)
  * and AutoregressiveDecoder.embed_input_symbols (decoders/autoregressive.py:269-272).
- * out[i,:] = table[ids[i],:] * (mask ? mask[i] : 1).  n = number of ids. */
+ * out[i,:] = table[ids[i],:] * (mask ? mask[i] : 1).  n = number of ids.  An id outside [0, vocab) gives a
+ * zero row (tf.gather on the GPU) and no gradient. */
 int nm_embed_fwd(const int64_t* ids, const float* table, const float* mask,
                  float* out, int64_t n, int64_t emb, int64_t vocab, void* stream);
 /* dtable[ids[i],:] += dout[i,:] * mask[i]  (dtable is accumulated into). */
@@ -519,6 +520,36 @@ int nm_ctc_loss_bwd(const float* logits, const int32_t* frames, const int64_t* l
                     void* stream);
 int nm_ctc_greedy_decode(const float* logits, const int32_t* frames, int merge_repeated, int64_t* ids,
                          int32_t* lengths, int64_t B, int64_t T, int64_t C, void* stream);
+
+/* ---- K17: rewards and sampling of the reinforcement-learning objectives ----------------------------------------
+ * nm_sentence_ngram_reward replaces the tf.py_func over sentence_bleu / sentence_gleu of
+ * trainers/self_critical_objective.py:124-231.  references [T_r,B] and hypotheses [T_h,B] are int64 token ids,
+ * element (t,b) at t*stride_t + b*stride_b (any strides); reward [B] fp32.  Per sentence and n = 1..4, n-grams are
+ * taken until the first window whose LAST token is </s> (2); <pad> before it is an ordinary token, and a row
+ * without </s> contributes every window.  A hypothesis n-gram is matched while fewer equal n-grams precede it in
+ * the hypothesis than the reference holds (clipped counts).
+ *   NM_REWARD_BLEU: 0 without hypothesis unigrams, else min(1, exp(1 - ref_len / hyp_1grams)) *
+ *     (m1 (m2+1)(m3+1)(m4+1) / (h1 (h2+1)(h3+1)(h4+1)))^(1/4), ref_len = tokens before the first </s>;
+ *   NM_REWARD_GLEU: min(sum m / sum h, sum m / sum r); 0 where either denominator is 0 (the reference's assert
+ *     fails there).
+ * Computed in fp64, rounded to fp32 once.  T_r, T_h <= NM_REWARD_MAX_LEN, otherwise NM_E_UNSUPPORTED. */
+#define NM_REWARD_BLEU 0
+#define NM_REWARD_GLEU 1
+#define NM_REWARD_MAX_LEN 2048
+int nm_sentence_ngram_reward(const int64_t* references, int64_t ref_stride_t, int64_t ref_stride_b,
+                             const int64_t* hypotheses, int64_t hyp_stride_t, int64_t hyp_stride_b, float* reward,
+                             int64_t T_r, int64_t T_h, int64_t B, int mode, void* stream);
+/* One draw per row of logits [rows,V] (row stride ldl >= V, or 0: every row reads the same logits) from
+ * softmax(logits / temperature): tf.multinomial of get_body (decoders/autoregressive.py:463-465,492-493) as the
+ * reference's RL sampling pass (trainers/rl_trainer.py:120-126) runs it.  Gumbel-max over Philox4x32-10 keyed by
+ * the runtime state {seed, step} (the one nm_dropout_apply reads), with the row, loop_step (< 65536) and
+ * sample_index (< 32768) in the counter: every row, loop step, sample and training step draws afresh, the same
+ * arguments draw the same symbols.  Column unk_index (>= 0) is never drawn.  Then the bookkeeping of get_body:
+ *   symbols[r] = finished_in[r] ? 0 : draw;  finished_out[r] = finished_in[r] | (symbols[r] == 2).
+ * finished_in / finished_out (u8, may alias, may be NULL). */
+int nm_sample_logits_step(const float* logits, int64_t ldl, float temperature, int64_t unk_index,
+                          const uint8_t* finished_in, int64_t* symbols, uint8_t* finished_out, const int64_t* state,
+                          int64_t loop_step, int64_t sample_index, int64_t rows, int64_t V, void* stream);
 
 #ifdef __cplusplus
 }

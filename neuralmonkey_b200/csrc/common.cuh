@@ -84,6 +84,27 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return red[0];
 }
 
+// Philox4x32-10 (Salmon et al., SC'11): counter-based random bits, shared by dropout (dropout.cu) and the
+// sampler of rl.cu.  Their counters occupy disjoint ranges of the third word (see the two files).
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+  constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
+    const uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += W0;
+    k.y += W1;
+  }
+  return c;
+}
+
+// The Philox key of a training step from the device state {seed, step} the runtime keeps.
+__device__ __forceinline__ uint2 philox_step_key(const int64_t* __restrict__ state) {
+  const uint64_t seed = (uint64_t)state[0], step = (uint64_t)state[1];
+  return make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32));
+}
+
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
 __device__ __forceinline__ float apply_act(float x, int act) {

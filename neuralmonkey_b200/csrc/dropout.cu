@@ -6,27 +6,14 @@
 // Random stream: key = seed, counter = (element index / 4, call site, step).  `state` is a device array
 // {seed, step}: the host bumps `step` once per training step (outside any captured graph), `site` numbers the
 // dropout calls of a step in program order - a CUDA graph that replays the step draws new masks each replay.
+// Sites stay below 2^31: the sampler of rl.cu owns the counters whose third word has its top bit set.
 #include "common.cuh"
 
 namespace nm {
 
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-  constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
-    const uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += W0;
-    k.y += W1;
-  }
-  return c;
-}
-
 __device__ __forceinline__ uint4 keep_bits(const int64_t* __restrict__ state, int64_t quad, uint32_t site) {
-  const uint64_t seed = (uint64_t)state[0], step = (uint64_t)state[1];
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32));
-  return philox4x32_10(make_uint4((uint32_t)quad, (uint32_t)((uint64_t)quad >> 32), site, (uint32_t)step), key);
+  return philox4x32_10(make_uint4((uint32_t)quad, (uint32_t)((uint64_t)quad >> 32), site, (uint32_t)state[1]),
+                       philox_step_key(state));
 }
 
 // MODE 0: y = keep ? x * scale : 0 (+ residual);  MODE 1: y = keep ? scale : 0 (the mask itself)

@@ -12,13 +12,19 @@ namespace nm {
 template <int VEC>
 __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ table,
                                  const float* __restrict__ mask, float* __restrict__ out,
-                                 int64_t n, int64_t emb) {
+                                 int64_t n, int64_t emb, int64_t vocab) {
   const int64_t per_row = emb / VEC;
   const int64_t total = n * per_row;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = i / per_row, c = (i - row * per_row) * VEC;
     const int64_t id = ids[row];
+    // an id outside the table (e.g. the argmax of a row of NaN logits) embeds as zeros, as tf.gather does on
+    // the GPU, instead of reading outside the table
+    if (id < 0 || id >= vocab) {
+      for (int k = 0; k < VEC; ++k) out[row * emb + c + k] = 0.f;
+      continue;
+    }
     const float m = mask ? mask[row] : 1.f;
     if (VEC == 4) {
       float4 v = *reinterpret_cast<const float4*>(table + id * emb + c);
@@ -32,13 +38,14 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* _
 
 __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ dout,
                                  const float* __restrict__ mask, float* __restrict__ dtable,
-                                 int64_t n, int64_t emb) {
+                                 int64_t n, int64_t emb, int64_t vocab) {
   const int64_t total = n * emb;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = i / emb, c = i - row * emb;
+    const int64_t id = ids[row];
     const float m = mask ? mask[row] : 1.f;
-    if (m != 0.f) atomicAdd(dtable + ids[row] * emb + c, dout[i] * m);
+    if (m != 0.f && id >= 0 && id < vocab) atomicAdd(dtable + id * emb + c, dout[i] * m);   // (ids outside: zeros)
   }
 }
 
@@ -301,9 +308,9 @@ int nm_embed_fwd(const int64_t* ids, const float* table, const float* mask, floa
   cudaStream_t s = (cudaStream_t)stream;
   const bool vec = (emb % 4 == 0) && (((uintptr_t)table | (uintptr_t)out) % 16 == 0);
   if (vec)
-    embed_fwd_kernel<4><<<grid_for(n * emb / 4, 256), 256, 0, s>>>(ids, table, mask, out, n, emb);
+    embed_fwd_kernel<4><<<grid_for(n * emb / 4, 256), 256, 0, s>>>(ids, table, mask, out, n, emb, vocab);
   else
-    embed_fwd_kernel<1><<<grid_for(n * emb, 256), 256, 0, s>>>(ids, table, mask, out, n, emb);
+    embed_fwd_kernel<1><<<grid_for(n * emb, 256), 256, 0, s>>>(ids, table, mask, out, n, emb, vocab);
   NM_LAUNCH_CHECK("nm_embed_fwd");
   return NM_OK;
 }
@@ -314,7 +321,7 @@ int nm_embed_bwd(const int64_t* ids, const float* dout, const float* mask, float
   NM_REQUIRE(n >= 0 && emb > 0 && vocab > 0, NM_E_INVALID, "nm_embed_bwd: bad sizes");
   if (n == 0) return NM_OK;
   embed_bwd_kernel<<<grid_for(n * emb, 256), 256, 0, (cudaStream_t)stream>>>(ids, dout, mask, dtable,
-                                                                             n, emb);
+                                                                             n, emb, vocab);
   NM_LAUNCH_CHECK("nm_embed_bwd");
   return NM_OK;
 }

@@ -13,7 +13,7 @@ Variants (SURVEY.md 8(f) N4, see nn/variants.py; GPU-verified by tests/test_gpu_
 or `rnn_cell="NematusGRU"` the context feeds the recurrence, so training steps through time with the
 same `_variant_step` the runtime uses (teacher-forced inputs), one set of T = 1 launches per step.
 """
-from typing import Any, List, NamedTuple, Tuple
+from typing import Any, Dict, List, NamedTuple, Tuple
 
 import torch
 
@@ -33,7 +33,7 @@ from neuralmonkey_b200.model.sequence import EmbeddedSequence
 from neuralmonkey_b200.model.stateful import Stateful
 from neuralmonkey_b200.nn.utils import dropout, dropout_mask
 from neuralmonkey_b200.nn.variants import LSTMCell, NematusGRUCell
-from neuralmonkey_b200.vocabulary import Vocabulary
+from neuralmonkey_b200.vocabulary import END_TOKEN_INDEX, START_TOKEN_INDEX, Vocabulary
 
 RNN_CELL_TYPES = ("NematusGRU", "GRU", "LSTM")
 
@@ -270,6 +270,71 @@ class Decoder(AutoregressiveDecoder):
     def train_rnn_outputs(self) -> torch.Tensor:
         """[time, batch, rnn_size] history of (dropped-out) cell outputs."""
         return self._train_pass[1].transpose(0, 1)
+
+    # -- the decoding loop under autograd (the reinforcement-learning objectives) ----------------------------
+    def differentiable_loop(self, sample: bool = False, temperature: float = 1.,
+                            sample_index: int = 0) -> Dict[str, torch.Tensor]:
+        """decoding_loop(train_mode=False, sample, temperature) as the reference's RL objectives differentiate it
+        (trainers/rl_trainer.py:120-140, self_critical_objective.py:56-92): the loop runs inside the training
+        graph, so decoder dropout is active in training and the gradient passes through the same masks that chose
+        the symbols.  Each step computes its output state with autograd through `_variant_step` (as the step-wise
+        training pass does), projects it to logits without autograd and chooses the next symbol: the first-index
+        argmax, or a draw from softmax(logits / temperature) (`ops.sample_logits_step`, `sample_index` selects an
+        independent stream); then symbols *= unfinished, finished |= symbols == </s> (get_body,
+        autoregressive.py:446-517).  The loop stops when every row has finished or after max_output_len steps.
+
+        Returns time-major {"states" [T,B,O] (differentiable), "symbols" [T,B], "argmax" [T,B] (the unmasked argmax
+        of the step's logits), "mask" [T,B] (not finished after the step)}; `loop_nll` gives the per-position
+        negative log-likelihoods of chosen symbols."""
+        if temperature <= 0:
+            raise ValueError("The softmax temperature must be positive")
+        dev = runtime.device()
+        symbols = torch.full((self.batch_size,), START_TOKEN_INDEX, dtype=torch.int64, device=dev)
+        finished = torch.zeros(self.batch_size, dtype=torch.bool, device=dev)
+        prev = self.initial_state
+        if self._rnn_cell_str == "LSTM":
+            prev = (prev, prev)
+
+        def attend(att, query):
+            ctx, w = att.attention_sequence(query.unsqueeze(1))
+            return ctx[:, 0], w
+
+        states, chosen, argmaxes, masks = [], [], [], []
+        for step in range(self.max_output_len):
+            out, prev, _ctx, _attended = self._variant_step(self.embed_input_symbols(symbols), prev, attend)
+            with torch.no_grad():
+                logits, _lse, argmax = self.state_to_logits(out.detach(), keep_logits=sample)
+                if sample:
+                    symbols, finished = ops.sample_logits_step(logits, temperature, finished, self._unk_index, step,
+                                                               sample_index)
+                else:
+                    symbols = argmax * (~finished).to(torch.int64)
+                    finished = finished | (symbols == END_TOKEN_INDEX)
+            states.append(out)
+            chosen.append(symbols)
+            argmaxes.append(argmax)
+            masks.append(~finished)
+            if bool(finished.all()):
+                break
+        return {"states": torch.stack(states, 0), "symbols": torch.stack(chosen, 0),
+                "argmax": torch.stack(argmaxes, 0), "mask": torch.stack(masks, 0)}
+
+    def loop_nll(self, states: torch.Tensor, targets: torch.Tensor, temperature: float = 1.):
+        """-log softmax(logits / temperature)[target] of states [T,B,O] (from `differentiable_loop`) at targets
+        [T,B]: one batched `ops.logits_xent`, differentiable in the states and the projection.  Returns
+        (nll [T,B], first-index argmax of the logits [T,B]).  Like the reference (autoregressive.py:492-493) the
+        temperature divides the whole projection; the -1e9 <unk> column is not divided, which changes nothing, as
+        its exponential is 0 either way."""
+        steps, bsz, dim = states.shape
+        w, b = self.decoding_w, self.decoding_b
+        if temperature != 1.:
+            w = w / temperature
+            b = b / temperature if b is not None else None
+        ones = torch.ones(steps * bsz, device=states.device, dtype=torch.float32)
+        nll, _lse, argmax, _ = ops.logits_xent(states.reshape(steps * bsz, dim), w, b,
+                                               targets.reshape(-1).contiguous(), ones, self._unk_index,
+                                               self._w_transposed)
+        return nll.view(steps, bsz), argmax.view(steps, bsz)
 
     # -- runtime: one step ----------------------------------------------------------------
     def get_initial_feedables(self):

@@ -1168,6 +1168,48 @@ def ctc_greedy_decode(logits: torch.Tensor, frames: torch.Tensor, merge_repeated
 
 
 # ---------------------------------------------------------------------------
+# K17 rewards and sampling of the reinforcement-learning objectives
+# ---------------------------------------------------------------------------
+REWARD_MODES = {"bleu": 0, "gleu": 1}
+
+
+def sentence_ngram_reward(references: torch.Tensor, hypotheses: torch.Tensor, mode: str) -> torch.Tensor:
+    """Index-based sentence BLEU or GLEU (trainers/self_critical_objective.py:124-231) of time-major int64 token
+    ids references [T_r, B] and hypotheses [T_h, B], any strides: [B] float32 on the device."""
+    if references.dim() != 2 or hypotheses.dim() != 2 or references.shape[1] != hypotheses.shape[1]:
+        raise ValueError("references and hypotheses must be [time, batch] with the same batch, got {} and {}"
+                         .format(tuple(references.shape), tuple(hypotheses.shape)))
+    if references.dtype != torch.int64 or hypotheses.dtype != torch.int64:
+        raise ValueError("token ids must be int64")
+    t_r, bsz = references.shape
+    t_h = hypotheses.shape[0]
+    reward = torch.empty(bsz, device=references.device, dtype=torch.float32)
+    call("nm_sentence_ngram_reward", ptr(references), references.stride(0), references.stride(1), ptr(hypotheses),
+         hypotheses.stride(0), hypotheses.stride(1), ptr(reward), t_r, t_h, bsz, REWARD_MODES[mode], lib.stream())
+    return reward
+
+
+def sample_logits_step(logits: torch.Tensor, temperature: float, finished: torch.Tensor, unk_index: int,
+                       loop_step: int, sample_index: int):
+    """One draw per row of logits [rows, V] (unit column stride) from softmax(logits / temperature), never column
+    `unk_index`, then get_body's bookkeeping: symbols = draw * ~finished, finished |= symbols == </s>.  The
+    random stream is the runtime's {seed, step} with (row, loop_step, sample_index) in the counter.
+    Returns (symbols [rows] int64, finished [rows] bool)."""
+    from neuralmonkey_b200 import runtime
+    rows, v = logits.shape
+    if logits.dtype != torch.float32 or logits.stride(1) != 1:
+        raise ValueError("sample_logits_step needs fp32 logits with unit column stride")
+    if finished.dtype != torch.bool or finished.shape != (rows,):
+        raise ValueError("finished must be bool [rows]")
+    symbols = torch.empty(rows, device=logits.device, dtype=torch.int64)
+    finished_out = torch.empty(rows, device=logits.device, dtype=torch.bool)
+    call("nm_sample_logits_step", ptr(logits), logits.stride(0), float(temperature), int(unk_index),
+         ptr(finished.contiguous()), ptr(symbols), ptr(finished_out), ptr(runtime.dropout_state()), int(loop_step),
+         int(sample_index), rows, v, lib.stream())
+    return symbols, finished_out
+
+
+# ---------------------------------------------------------------------------
 # K12 frozen VGG stack primitives (forward only)
 # ---------------------------------------------------------------------------
 def conv3x3_bias_relu(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:

@@ -54,6 +54,12 @@ class GenericTrainer(GraphExecutor, Feedable):
         self.batches_per_update = 1
         if clip_norm is not None and clip_norm <= 0.0:
             raise ValueError("clip_norm must be positive")
+        if use_cuda_graph:
+            eager = [obj.name for obj in objectives if not getattr(obj, "graph_capturable", True)]
+            if eager:
+                # their loop length and rewards depend on the data: a captured step could not replay them
+                raise ValueError("use_cuda_graph=True cannot capture the step of objective(s) {}: their decoding "
+                                 "loops stop and score on the host".format(", ".join(eager)))
 
     @property
     def global_step(self) -> int:
