@@ -145,14 +145,14 @@ __global__ void xent_bwd_kernel(const float* __restrict__ logits, const int64_t*
                                 const float* __restrict__ weights, const float* __restrict__ lse,
                                 const float* __restrict__ scale, float* __restrict__ dlogits,
                                 int64_t V, int64_t ldl) {
-  const int64_t row = blockIdx.y;
+  const int64_t row = blockIdx.x;  // rows on grid.x (up to 2^31-1), column blocks on grid.y
   const float wgt = (weights ? weights[row] : 1.f) * scale[0];
   const float l = lse[row];
   const int64_t tgt = targets[row];
   const float* lr = logits + row * ldl;
   float* dr = dlogits + row * ldl;
-  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < V;
-       c += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t c = blockIdx.y * (int64_t)blockDim.x + threadIdx.x; c < V;
+       c += (int64_t)gridDim.y * blockDim.x) {
     const float p = expf(lr[c] - l);
     dr[c] = (p - (c == tgt ? 1.f : 0.f)) * wgt;
   }
@@ -160,10 +160,10 @@ __global__ void xent_bwd_kernel(const float* __restrict__ logits, const int64_t*
 
 __global__ void log_softmax_kernel(const float* __restrict__ logits, const float* __restrict__ lse,
                                    float* __restrict__ out, int64_t V, int64_t ldl) {
-  const int64_t row = blockIdx.y;
+  const int64_t row = blockIdx.x;  // as xent_bwd_kernel
   const float l = lse[row];
-  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < V;
-       c += (int64_t)gridDim.x * blockDim.x)
+  for (int64_t c = blockIdx.y * (int64_t)blockDim.x + threadIdx.x; c < V;
+       c += (int64_t)gridDim.y * blockDim.x)
     out[row * V + c] = logits[row * ldl + c] - l;
 }
 
@@ -235,9 +235,9 @@ int nm_xent_bwd(const float* logits, const int64_t* targets, const float* weight
                 const float* scale, float* dlogits, int64_t M, int64_t V, int64_t ldl, void* stream) {
   NM_REQUIRE(logits && targets && lse && scale && dlogits, NM_E_INVALID, "nm_xent_bwd: null pointer");
   NM_REQUIRE(M >= 0 && V > 0 && ldl >= V, NM_E_INVALID, "nm_xent_bwd: bad sizes");
-  NM_REQUIRE(M <= 65535, NM_E_UNSUPPORTED, "nm_xent_bwd: M > 65535 rows per call");
+  NM_REQUIRE(M <= 0x7fffffffLL, NM_E_UNSUPPORTED, "nm_xent_bwd: M > 2^31-1 rows per call");
   if (M == 0) return NM_OK;
-  dim3 grid((unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64), (unsigned)M);
+  dim3 grid((unsigned)M, (unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64));
   xent_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, targets, weights, lse, scale,
                                                           dlogits, V, ldl);
   NM_LAUNCH_CHECK("nm_xent_bwd");
@@ -248,9 +248,9 @@ int nm_log_softmax(const float* logits, const float* lse, float* logprobs, int64
                    int64_t ldl, void* stream) {
   NM_REQUIRE(logits && lse && logprobs, NM_E_INVALID, "nm_log_softmax: null pointer");
   NM_REQUIRE(M >= 0 && V > 0 && ldl >= V, NM_E_INVALID, "nm_log_softmax: bad sizes");
-  NM_REQUIRE(M <= 65535, NM_E_UNSUPPORTED, "nm_log_softmax: M > 65535 rows per call");
+  NM_REQUIRE(M <= 0x7fffffffLL, NM_E_UNSUPPORTED, "nm_log_softmax: M > 2^31-1 rows per call");
   if (M == 0) return NM_OK;
-  dim3 grid((unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64), (unsigned)M);
+  dim3 grid((unsigned)M, (unsigned)(ceil_div(V, 256) < 64 ? ceil_div(V, 256) : 64));
   log_softmax_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, lse, logprobs, V, ldl);
   NM_LAUNCH_CHECK("nm_log_softmax");
   return NM_OK;

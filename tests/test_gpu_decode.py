@@ -186,7 +186,8 @@ def test_fused_greedy_against_the_oracle_bit_exact_symbols():
 
 
 @pytest.mark.parametrize("cfg,backend,bsz,beam,alpha", [(TOY, "simt", 1, 3, 0.6), (TOY, "simt", 4, 4, 1.0),
-                                                        (MID, "simt", 5, 8, 0.0), (MID, "auto", 3, 5, 0.6)])
+                                                        (MID, "simt", 5, 8, 0.0), (MID, "auto", 3, 5, 0.6),
+                                                        (MID, "simt", 3, 16, 0.6)])
 def test_fused_beam_search_equals_the_stepwise_loop(cfg, backend, bsz, beam, alpha):
     from neuralmonkey_b200 import ops
     from neuralmonkey_b200.decoders import BeamSearchDecoder
@@ -211,7 +212,11 @@ def test_fused_beam_search_equals_the_stepwise_loop(cfg, backend, bsz, beam, alp
                 assert max_abs(a.scores, b.scores) < 1e-5
                 assert max_abs(got.last_search_state.logprob_sum, base.last_search_state.logprob_sum) < 1e-4
             else:
-                assert a.token_ids.shape == b.token_ids.shape or True
+                # after a near-tie the two paths may pick other words and stop at other steps; the layout
+                # [steps + 1, batch, beam] with at most max_steps = 9 search steps, and the id range, still hold
+                assert a.token_ids.shape[1:] == b.token_ids.shape[1:] == (bsz, beam)
+                assert 1 <= a.token_ids.shape[0] <= 10 and 1 <= b.token_ids.shape[0] <= 10
+                assert 0 <= int(a.token_ids.min()) and int(a.token_ids.max()) < cfg["vt"]
                 assert max_abs(a.scores[:, 0], b.scores[:, 0]) < 5e-2
     finally:
         ops.set_gemm_backend("auto")
