@@ -281,6 +281,11 @@ int nm_gemm_f16(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, c
  * transposed copies. */
 int nm_gemm_f16_tn(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16,
                    int64_t ldb, float* C, int64_t ldc, const float* alpha_dev, float beta, void* stream);
+/* nm_gemm_f16_tn on at most max_ctas SMs (<= 0: all of them), leaving the others to work issued concurrently
+ * on other streams: the product runs one persistent CTA per SM it is given, which no other kernel can share. */
+int nm_gemm_f16_tn_ctas(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16,
+                        int64_t ldb, float* C, int64_t ldc, const float* alpha_dev, float beta, int max_ctas,
+                        void* stream);
 int nm_logits_xent_fwd16(const void* X16, int64_t ldx, const void* WT16, int64_t ldw, const float* b,
                          int64_t unk_index, const int64_t* targets, const float* weights, float* lse,
                          float* xent, int64_t* argmax, float* part, float* logits_out, int64_t ldl,

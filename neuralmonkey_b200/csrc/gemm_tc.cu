@@ -8,13 +8,14 @@
 //     swizzle.  K-major operands arrive by cp.async.bulk.tensor (OOB rows / cols as zeros);
 //     wgmma takes TF32 operands K-major only, so MN-major TF32 operands (reduction dim strided)
 //     are loaded by the producer warpgroup's threads and written K-major (transposed, rounded to
-//     TF32) into the same layout; MN-major fp16 operands arrive by TMA as they are stored and
-//     wgmma reads them transposed;
+//     TF32) into the same layout;
 //   * after the main loop the accumulators go through shared memory (the ring is free by then)
 //     and the epilogue warps read whole 32-column row chunks: one thread = one output row;
 //   * epilogues: dense (bias/activation/accumulate), and the fused vocabulary
 //     cross-entropy forward (online softmax partials + argmax + target logit) and
-//     backward (softmax - onehot), which never materialise fp32 logits twice.
+//     backward (softmax - onehot), which never materialise fp32 logits twice.  The fp16
+//     instances carry the cross-entropy epilogues only (K > XENT16_MAX_K); the dense fp16
+//     products run on the persistent kernel of gemm16.cu.
 //
 // Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" of the wgmma section.
 #include <cuda.h>
@@ -260,20 +261,6 @@ __device__ __forceinline__ void epilogue_chunk_atomic(const TcEpilogue& e, const
 // ---------------------------------------------------------------------------
 // epilogues of the fp16-operand instances (ESZ == 2)
 // ---------------------------------------------------------------------------
-// Transposed store of a warp's 32x32 chunk: lane = row, so for one column the 32 lanes write 32
-// consecutive elements of the transposed matrix - a full segment without any staging.
-__device__ __forceinline__ void store32_transposed(float* __restrict__ ct, int64_t ldt, int64_t row, int col0,
-                                                   int64_t M, int ncols, const float (&x)[32], float beta) {
-  if (row >= M) return;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    if (j < ncols) {
-      float* dst = ct + (int64_t)(col0 + j) * ldt + row;
-      *dst = (beta != 0.f) ? (x[j] + *dst) : x[j];
-    }
-  }
-}
-
 // Row-major fp16 store of a warp's 32x32 chunk through the per-warp staging tile (32 rows x 64 B,
 // 16-byte slots XOR-swizzled): every store instruction then writes eight full 64-byte row segments.
 __device__ __forceinline__ void store32_half_coalesced(float* __restrict__ stage, __half* __restrict__ C,
@@ -337,28 +324,6 @@ __device__ __forceinline__ void epilogue_chunk_xent_bwd16(const TcEpilogue& e, c
     for (int j = 0; j < 32; ++j)
       if (j < ncols) c16[row * ext.ldc16 + col0 + j] = __float2half_rn(x[j]);
   }
-}
-
-// TC_EPI_DENSE of the fp16 instances: C (or C^T) = alpha * row_scale[m] * acc + bias (+ C).
-__device__ __forceinline__ void epilogue_chunk_dense16(const TcEpilogue& e, const TcExt& ext, float (&x)[32],
-                                                       int64_t row, int col0, int64_t M, int N, float factor,
-                                                       bool vec_ok, float* __restrict__ stage, int lane,
-                                                       RowStats& st) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) x[j] *= factor;
-  if (!ext.transposed) {
-    epilogue_chunk<TC_EPI_DENSE>(e, x, row, col0, M, N, st, -1, 0.f, 0.f, vec_ok, stage, lane);
-    return;
-  }
-  if (col0 >= N) return;
-  const int ncols = min(32, N - col0);
-  if (e.bias) {
-    float b[32];
-    load_bias32(e.bias, col0, ncols, b);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) x[j] += b[j];
-  }
-  store32_transposed(e.C, e.ldc, row, col0, M, ncols, x, e.beta);
 }
 
 // ---------------------------------------------------------------------------
@@ -519,11 +484,11 @@ struct TcOperand {
   int64_t rows, cols, ld;
 };
 
-// One k-block of an MN-major operand: R MN rows x 128 bytes of K, written K-major into the 128-byte swizzle
-// (16-byte chunk c of row m at chunk c ^ (m & 7)).  An item is one 32-bit word of a row (one tf32 or two fp16
-// k values); a warp covers 8 rows x 4 words, so the shared-memory stores hit 32 different banks and the loads of
-// one k row are 8 consecutive MN elements.  Called by the 128 threads of the producer warpgroup.
-template <int ESZ, int R>
+// One k-block of an MN-major TF32 operand: R MN rows x 32 k values, written K-major into the 128-byte swizzle
+// (16-byte chunk c of row m at chunk c ^ (m & 7)).  An item is one 32-bit word of a row; a warp covers 8 rows x
+// 4 words, so the shared-memory stores hit 32 different banks and the loads of one k row are 8 consecutive MN
+// elements.  Called by the 128 threads of the producer warpgroup.
+template <int R>
 __device__ __forceinline__ void load_mn_tile(uint8_t* __restrict__ dst, const TcOperand& op, int64_t k_row0,
                                              int64_t mn0, int tid) {
   constexpr int PER = R * 32 / 128;
@@ -535,20 +500,9 @@ __device__ __forceinline__ void load_mn_tile(uint8_t* __restrict__ dst, const Tc
     const int word = (rest / (R / 8)) * 4 + b;
     const int64_t col = mn0 + m;
     const bool col_ok = col < op.cols;
-    uint32_t packed;
-    if constexpr (ESZ == 4) {
-      const int64_t r = k_row0 + word;
-      const float* f = reinterpret_cast<const float*>(op.ptr);
-      packed = to_tf32((col_ok && r < op.rows) ? __ldg(f + r * op.ld + col) : 0.f);
-    } else {
-      const int64_t r = k_row0 + 2 * word;
-      const __half* h = reinterpret_cast<const __half*>(op.ptr);
-      const __half zero = __float2half_rn(0.f);
-      const __half lo = (col_ok && r < op.rows) ? h[r * op.ld + col] : zero;
-      const __half hi = (col_ok && r + 1 < op.rows) ? h[(r + 1) * op.ld + col] : zero;
-      const __half2 v = __halves2half2(lo, hi);
-      packed = *reinterpret_cast<const uint32_t*>(&v);
-    }
+    const int64_t r = k_row0 + word;
+    const float* f = reinterpret_cast<const float*>(op.ptr);
+    const uint32_t packed = to_tf32((col_ok && r < op.rows) ? __ldg(f + r * op.ld + col) : 0.f);
     *reinterpret_cast<uint32_t*>(dst + m * 128 + (((word >> 2) ^ (m & 7)) << 4) + ((word & 3) << 2)) = packed;
   }
 }
@@ -561,9 +515,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                TcOperand opa, TcOperand opb, int64_t M, int64_t N, int64_t K, TcEpilogue epi, int splits,
                int kb_per_split, TcExt ext, TcBatch bt) {
   static_assert(ESZ == 2 || MODE != TC_EPI_XENT_BWD16, "the fp16 epilogue belongs to the fp16 instances");
+  static_assert(ESZ == 4 || (!A_MN && !B_MN && (MODE == TC_EPI_XENT_FWD || MODE == TC_EPI_XENT_BWD16)),
+                "fp16 instances: K-major operands, cross-entropy epilogues");
   constexpr int BK = 128 / ESZ;                // elements per 128-byte k-block
-  constexpr bool MN16 = ESZ == 2 && A_MN && B_MN;   // fp16, both MN-major: TMA boxes, transposed wgmma operands
-  constexpr bool A_MANUAL = A_MN && !MN16, B_MANUAL = B_MN && !MN16;
+  constexpr bool A_MANUAL = A_MN, B_MANUAL = B_MN;
   constexpr bool MANUAL = A_MANUAL || B_MANUAL;      // the producer threads write (some of) the tiles
   using Cfg = TcCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
@@ -628,23 +583,16 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       if (ptid == 0) {
         constexpr uint32_t TX = (A_MANUAL ? 0u : (uint32_t)TC_A_BYTES) + (B_MANUAL ? 0u : (uint32_t)Cfg::B_BYTES);
         if (TX) mbar_expect_tx_only(full_bar(s), TX);
-        if constexpr (MN16) {   // boxes {64 MN elements, one k-block of rows}, 8 KB each
-#pragma unroll
-          for (int j = 0; j < TC_BM / 64; ++j)
-            tma_load_2d(a_dst + j * 8192, &map_a, full_bar(s), m0 + a_col + 64 * j, k0 + a_row);
-#pragma unroll
-          for (int j = 0; j < BN / 64; ++j)
-            tma_load_2d(b_dst + j * 8192, &map_b, full_bar(s), n0 + b_col + 64 * j, k0 + b_row);
-        } else if (!A_MN) {
+        if (!A_MN) {
           tma_load_2d(a_dst, &map_a, full_bar(s), k0 + a_col, m0 + a_row);  // box {one k-block, 128 rows}
         }
-        if (!B_MN) {   // (MN16 loaded it above)
+        if (!B_MN) {
           tma_load_2d(b_dst, &map_b, full_bar(s), k0 + b_col, n0 + b_row);  // box {one k-block, BN rows}
         }
       }
       uint8_t* ring = smem + s * Cfg::STAGE_BYTES;
-      if constexpr (A_MANUAL) load_mn_tile<ESZ, TC_BM>(ring, opa, k0 + a_row, m0 + a_col, ptid);
-      if constexpr (B_MANUAL) load_mn_tile<ESZ, BN>(ring + TC_A_BYTES, opb, k0 + b_row, n0 + b_col, ptid);
+      if constexpr (A_MANUAL) load_mn_tile<TC_BM>(ring, opa, k0 + a_row, m0 + a_col, ptid);
+      if constexpr (B_MANUAL) load_mn_tile<BN>(ring + TC_A_BYTES, opb, k0 + b_row, n0 + b_col, ptid);
       // the generic-proxy stores above become visible to wgmma (async proxy) before the arrive
       if constexpr (MANUAL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_arrive(full_bar(s));
@@ -659,16 +607,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   for (int kb = 0; kb < num_kb; ++kb) {
     const int s = kb % STAGES;
     mbar_wait(full_bar(s), (uint32_t)((kb / STAGES) & 1));
-    const uint32_t a_addr = smem_base + s * Cfg::STAGE_BYTES + wg * 64 * 128;   // K-major: 64 rows; MN16: one box
+    const uint32_t a_addr = smem_base + s * Cfg::STAGE_BYTES + wg * 64 * 128;   // this warpgroup's 64 rows
     const uint32_t b_addr = smem_base + s * Cfg::STAGE_BYTES + TC_A_BYTES;
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if constexpr (MN16)
-        Wgmma<BN, 2, true>::mma(acc, gmma_desc_sw128_mn(a_addr + k * 2048), gmma_desc_sw128_mn(b_addr + k * 2048));
-      else
-        Wgmma<BN, ESZ>::mma(acc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32));
-    }
+    for (int k = 0; k < 4; ++k)
+      Wgmma<BN, ESZ>::mma(acc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32));
     wgmma_commit();
     wgmma_wait<1>();                           // the previous k-block's products are done with their stage
     wgmma_fence_operands(acc);
@@ -722,11 +666,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       row_w = epi.weights ? epi.weights[row] : 1.f;
     }
   }
-  float factor16 = 1.f;
-  if (ESZ == 2 && MODE == TC_EPI_DENSE) {
-    if (ext.alpha) factor16 = ext.alpha[0];
-    if (ext.row_scale && row < M) factor16 *= ext.row_scale[row];
-  }
   if constexpr (MODE == TC_EPI_SOFTMAX || MODE == TC_EPI_DSOFTMAX) {
     // whole rows per thread: the first warp of each quadrant does the tile (a handful of columns)
     if (half == 0) attn_epilogue<MODE>(epi, bt, crow, (int)row, (int)M, n32, prob_o, prob, c_off, stage, lane);
@@ -741,9 +680,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       if constexpr (MODE == TC_EPI_XENT_BWD16) {
         epilogue_chunk_xent_bwd16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, target, row_lse2,
                                   row_w, stage, lane);
-      } else if constexpr (ESZ == 2 && MODE == TC_EPI_DENSE) {
-        epilogue_chunk_dense16(epi, ext, v, row, (int)(tn * BN) + c * 32, M, n32, factor16, vec_ok,
-                               stage, lane, st);
       } else {
         if (MODE == TC_EPI_DENSE && splits > 1)
           epilogue_chunk_atomic(epi, v, row, (int)(tn * BN) + c * 32, M, n32, split == 0,
@@ -859,8 +795,7 @@ static int launch_tiles(const CUtensorMap& ma, const CUtensorMap& mb, const TcOp
 }
 
 // launch_tiles for the tile width bn.  Only the widths each kind of product uses are instantiated: dense products
-// 64, 128, 160 and 256 columns (fp16 with both operands MN-major: no 160), the vocabulary cross-entropy
-// TC_XENT_BN, the attention epilogues 128.
+// 64, 128, 160 and 256 columns, the vocabulary cross-entropy TC_XENT_BN, the attention epilogues 128.
 template <bool A_MN, bool B_MN, int MODE, int ESZ>
 static int launch_bn(int bn, const CUtensorMap& ma, const CUtensorMap& mb, const TcOperand& oa, const TcOperand& ob,
                      int64_t M, int64_t N, int64_t K, const TcEpilogue& epi, int splits, int kb_per_split,
@@ -878,7 +813,7 @@ static int launch_bn(int bn, const CUtensorMap& ma, const CUtensorMap& mb, const
                                                         s, name);
       break;
     case 160:
-      if constexpr (dense && !(ESZ == 2 && A_MN))
+      if constexpr (dense)
         return launch_tiles<160, A_MN, B_MN, MODE, ESZ>(ma, mb, oa, ob, M, N, K, epi, splits, kb_per_split, ext, bt,
                                                         s, name);
       break;
@@ -1023,31 +958,13 @@ static int check_f16_operands(const char* name, int64_t M, int64_t N, int64_t K,
   return NM_OK;
 }
 
-int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
-                        int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
-  // A stored [K, M] (row pitch lda), B stored [K, N] (row pitch ldb): both MN-major
-  int rc = check_f16_operands("tc_gemm16_mn", M, N, K, A, lda, B, ldb);
-  if (rc) return rc;
-  NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16_mn: dense epilogue only");
-  CUtensorMap ma, mb;   // [K, M] and [K, N] as stored, boxes of 64 columns x one 64-row k-block
-  rc = make_map16(&ma, A, K, M, lda, 64);
-  if (rc) return rc;
-  rc = make_map16(&mb, B, K, N, ldb, 64);
-  if (rc) return rc;
-  const TcOperand oa{A, K, M, lda}, ob{B, K, N, ldb};
-  int bn = 256;
-  if (N <= 64) bn = 64;
-  else if (N <= 128) bn = 128;
-  else if (ceil_div(M, TC_BM) * ceil_div(N, 256) < sm_count()) bn = 128;
-  return launch_bn<true, true, TC_EPI_DENSE, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
-                                                "tc_gemm_kernel(fp16)");
-}
-
 int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s) {
   int rc = check_f16_operands("tc_gemm16", M, N, K, A, lda, B, ldb);
   if (rc) return rc;
-  const int bn = (epi.mode == TC_EPI_DENSE) ? pick_bn(M, N, K) : TC_XENT_BN;
+  NM_REQUIRE(epi.mode == TC_EPI_XENT_FWD || epi.mode == TC_EPI_XENT_BWD16, NM_E_INVALID,
+             "tc_gemm16: unsupported epilogue %d", epi.mode);
+  const int bn = TC_XENT_BN;
   CUtensorMap ma, mb;
   TcOperand oa, ob;
   rc = make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 2);
@@ -1057,11 +974,8 @@ int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda
   const char* name = "tc_gemm_kernel(fp16)";
   if (epi.mode == TC_EPI_XENT_FWD)
     return launch_bn<false, false, TC_EPI_XENT_FWD, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s, name);
-  if (epi.mode == TC_EPI_XENT_BWD16)
-    return launch_bn<false, false, TC_EPI_XENT_BWD16, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
-                                                         name);
-  NM_REQUIRE(epi.mode == TC_EPI_DENSE, NM_E_INVALID, "tc_gemm16: unsupported epilogue %d", epi.mode);
-  return launch_bn<false, false, TC_EPI_DENSE, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s, name);
+  return launch_bn<false, false, TC_EPI_XENT_BWD16, 2>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, ext, TcBatch{}, s,
+                                                       name);
 }
 
 }  // namespace nm

@@ -39,9 +39,6 @@ struct TcEpilogue {
 struct TcExt {
   void* C16;               // xent_bwd16: [M,N] fp16, row pitch ldc16 (elements)
   int64_t ldc16;
-  const float* alpha;      // dense: device scalar multiplying the accumulator (null: 1)
-  const float* row_scale;  // dense: [M] per-row factor (null: 1)
-  int transposed;          // dense: store D^T - element (m, n) goes to C[n * ldc + m]
 };
 
 // Many small products in one launch: problem p = (o, i), o < count / inner, i < inner (sentence, head), all of the
@@ -96,14 +93,9 @@ int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, cons
                    int64_t lda, const float* B, int64_t ldb, const TcEpilogue& epi, cudaStream_t s);
 
 // The same product with fp16 operands, both K-major: A is [M,K] (row pitch lda), B is [N,K] (row pitch
-// ldb), pitches multiples of 8 elements, bases 16-byte aligned.  epi.mode: TC_EPI_DENSE (with `ext`),
-// TC_EPI_XENT_FWD or TC_EPI_XENT_BWD16.
+// ldb), pitches multiples of 8 elements, bases 16-byte aligned.  epi.mode: TC_EPI_XENT_FWD or
+// TC_EPI_XENT_BWD16 (the dense fp16 products are nm_gemm_f16 / nm_gemm_f16_tn, gemm16.cu).
 int tc_gemm16_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s);
-
-// The same with both operands MN-major (reduction dimension strided): A is [K,M] (row pitch lda), B is
-// [K,N] (row pitch ldb) - weight-gradient products X^T . dY without transposed copies.  Dense epilogue.
-int tc_gemm16_mn_launch(int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
-                        int64_t ldb, const TcEpilogue& epi, const TcExt& ext, cudaStream_t s);
 
 }  // namespace nm

@@ -7,8 +7,8 @@
 // UNNORMALISED ((softmax - onehot) * mask, values in [-1, 1]: fp16 then has TF32's 10 mantissa bits;
 // tools/fp16_dlogits_study.py), row-major, and every product is an fp16 wgmma GEMM:
 //     logits  = X16 [M,K]   . WT16 [V,K]^T          forward, and the recompute of the backward (xent16_kernel)
-//     dX      = dl16 [M,V]  . W16  [K,V]^T           * row_scale[m]                           (nm_gemm_f16)
-//     dW      = XS16 [M,K+1]^T . dl16 [M,V]         * alpha, MN-major operands               (nm_gemm_f16_tn)
+//     dX      = dl16 [M,V]  . W16  [K,V]^T           * row_scale[m]                (nm_gemm_f16, gemm16.cu)
+//     dW      = XS16 [M,K+1]^T . dl16 [M,V]         * alpha, MN-major operands    (nm_gemm_f16_tn, gemm16.cu)
 // The upstream per-row gradient is applied in fp32 in the consumers' epilogues.
 //
 // xent16_kernel: a persistent CTA per SM works through a contiguous range of 64 x 256 output tiles, row tiles
@@ -446,43 +446,6 @@ int nm_cast_f16(const float* src, int64_t ld_src, void* dst, int64_t ld_dst, int
   }
   NM_LAUNCH_CHECK("nm_cast_f16");
   return NM_OK;
-}
-
-int nm_gemm_f16(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16, int64_t ldb,
-                float* C, int64_t ldc, const float* alpha_dev, const float* row_scale, float beta,
-                int transposed, void* stream) {
-  NM_REQUIRE(A16 && B16 && C, NM_E_INVALID, "nm_gemm_f16: null pointer");
-  NM_REQUIRE(beta == 0.f || beta == 1.f, NM_E_INVALID, "nm_gemm_f16: beta must be 0 or 1");
-  NM_REQUIRE(lda >= K && ldb >= K && ldc >= (transposed ? M : N), NM_E_INVALID, "nm_gemm_f16: bad pitches");
-  TcEpilogue epi{};
-  epi.mode = TC_EPI_DENSE;
-  epi.C = C;
-  epi.ldc = ldc;
-  epi.act = NM_ACT_NONE;
-  epi.beta = beta;
-  epi.unk_index = -1;
-  TcExt ext{};
-  ext.alpha = alpha_dev;
-  ext.row_scale = row_scale;
-  ext.transposed = transposed;
-  return tc_gemm16_launch(M, N, K, A16, lda, B16, ldb, epi, ext, (cudaStream_t)stream);
-}
-
-int nm_gemm_f16_tn(int64_t M, int64_t N, int64_t K, const void* A16, int64_t lda, const void* B16, int64_t ldb,
-                   float* C, int64_t ldc, const float* alpha_dev, float beta, void* stream) {
-  NM_REQUIRE(A16 && B16 && C, NM_E_INVALID, "nm_gemm_f16_tn: null pointer");
-  NM_REQUIRE(beta == 0.f || beta == 1.f, NM_E_INVALID, "nm_gemm_f16_tn: beta must be 0 or 1");
-  NM_REQUIRE(lda >= M && ldb >= N && ldc >= N, NM_E_INVALID, "nm_gemm_f16_tn: bad pitches");
-  TcEpilogue epi{};
-  epi.mode = TC_EPI_DENSE;
-  epi.C = C;
-  epi.ldc = ldc;
-  epi.act = NM_ACT_NONE;
-  epi.beta = beta;
-  epi.unk_index = -1;
-  TcExt ext{};
-  ext.alpha = alpha_dev;
-  return tc_gemm16_mn_launch(M, N, K, A16, lda, B16, ldb, epi, ext, (cudaStream_t)stream);
 }
 
 int nm_logits_xent_bwd16(const void* X16, int64_t ldx, const void* WT16, int64_t ldw, const float* b,

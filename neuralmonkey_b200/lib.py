@@ -141,7 +141,7 @@ def call(name: str, *args) -> None:
         if name == "nm_gemm":  # split the projection calls by shape in the breakdown
             key = "nm_gemm[{}{} {}x{}x{}]".format("T" if args[0] else "N", "T" if args[1] else "N",
                                                  args[2], args[3], args[4])
-        elif name in ("nm_gemm_f16", "nm_gemm_f16_tn"):  # fp16 operands: M x N x K are the first three arguments
+        elif name in ("nm_gemm_f16", "nm_gemm_f16_tn", "nm_gemm_f16_tn_ctas"):  # fp16 operands: M x N x K are the first three arguments
             key = "{}[{}x{}x{}]".format(name, args[0], args[1], args[2])
         _profile.setdefault(key, []).append((ev0, ev1))
     else:
