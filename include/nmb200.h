@@ -365,8 +365,8 @@ int nm_mha_bwd(const float* q, const float* k, const float* v,
                int64_t Tq, int64_t Tk, int64_t heads, int64_t dh, void* stream);
 /* The same with attention-weight dropout (attention/scaled_dot_product.py:208-214): drop_mask
  * [B, heads, Tq, Tk] holds 0 or 1/keep_prob; context = (softmax * drop_mask) . V, while `probs`
- * keeps the undropped softmax (what the softmax backward needs).  Tiled kernels only
- * (dh % 8 == 0, dh <= 128, 8 <= Tq <= 256, Tk <= 256), otherwise NM_E_UNSUPPORTED. */
+ * keeps the undropped softmax (what the softmax backward needs).  Supported wherever nm_mha_fwd /
+ * nm_mha_bwd are: both the tiled and the row kernels apply the mask. */
 int nm_mha_fwd_drop(const float* q, const float* k, const float* v, const float* key_mask, int causal,
                     const float* drop_mask, float* out, float* probs, int64_t B, int64_t Tq,
                     int64_t Tk, int64_t heads, int64_t dh, void* stream);

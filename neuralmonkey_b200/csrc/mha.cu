@@ -6,7 +6,9 @@
 //
 // Two implementations: tiled kernels (below) for training shapes - one CTA per (32 query rows,
 // head, sentence) with the head's K/V resident in shared memory - and the original row kernels
-// (one CTA per query position) for single-query decoding steps and odd head sizes.
+// (one CTA per query position) for everything else: single-query decoding steps, fewer than 8
+// queries, odd or wide head sizes, more than 256 positions.  Both families take the attention-weight
+// dropout mask (DROP below), so dropout works at every shape the row kernels' shared memory allows.
 #include "common.cuh"
 
 namespace nm {
@@ -14,11 +16,14 @@ namespace nm {
 constexpr int MHA_THREADS = 128;
 constexpr float MHA_MASK = -1e9f;
 
-// dynamic smem: qs[dh] | e[Tk]
+// dynamic smem: qs[dh] | e[Tk].  DROP: as in mha_fwd_tile_kernel - the context is (p * drop) . V,
+// `probs` keeps the undropped p.
+template <bool DROP = false>
 __global__ void __launch_bounds__(MHA_THREADS)
 mha_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                const float* __restrict__ key_mask, int causal, float* __restrict__ out,
-               float* __restrict__ probs, int Tq, int Tk, int heads, int dh) {
+               float* __restrict__ probs, int Tq, int Tk, int heads, int dh,
+               const float* __restrict__ drop) {
   extern __shared__ float smem[];
   __shared__ float red[32];
   float* qs = smem;
@@ -51,9 +56,10 @@ mha_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, const f
   }
   const float s = block_sum(lsum, red);
   float* pr = probs + (((int64_t)b * heads + h) * Tq + tq) * Tk;
+  const float* dr = DROP ? drop + (((int64_t)b * heads + h) * Tq + tq) * Tk : nullptr;
   for (int tk = threadIdx.x; tk < Tk; tk += MHA_THREADS) {
     const float p = e[tk] / s;
-    e[tk] = p;
+    e[tk] = DROP ? p * dr[tk] : p;
     pr[tk] = p;
   }
   __syncthreads();
@@ -65,12 +71,14 @@ mha_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, const f
   }
 }
 
-// backward A: per query row: dE (pre-mask gradient) and dq.  smem: dos[dh] | de[Tk]
+// backward A: per query row: dE (pre-mask gradient) and dq.  smem: dos[dh] | de[Tk].
+// DROP: d(softmax) = drop * (dO . V), and the row sum and dE are formed from it.
+template <bool DROP = false>
 __global__ void __launch_bounds__(MHA_THREADS)
 mha_bwd_q_kernel(const float* __restrict__ k, const float* __restrict__ v,
                  const float* __restrict__ key_mask, int causal, const float* __restrict__ probs,
                  const float* __restrict__ dout, float* __restrict__ dq, float* __restrict__ de_out,
-                 int Tq, int Tk, int heads, int dh) {
+                 int Tq, int Tk, int heads, int dh, const float* __restrict__ drop) {
   extern __shared__ float smem[];
   __shared__ float red[32];
   float* dos = smem;
@@ -81,11 +89,13 @@ mha_bwd_q_kernel(const float* __restrict__ k, const float* __restrict__ v,
     dos[d] = dout[((int64_t)b * Tq + tq) * D + h * dh + d];
   __syncthreads();
   const float* pr = probs + (((int64_t)b * heads + h) * Tq + tq) * Tk;
+  const float* dr = DROP ? drop + (((int64_t)b * heads + h) * Tq + tq) * Tk : nullptr;
   float lsum = 0.f;
   for (int tk = threadIdx.x; tk < Tk; tk += MHA_THREADS) {
     const float* vr = v + ((int64_t)b * Tk + tk) * D + h * dh;
     float dp = 0.f;
     for (int d = 0; d < dh; ++d) dp = fmaf(dos[d], vr[d], dp);
+    if (DROP) dp *= dr[tk];
     de[tk] = dp;
     lsum += dp * pr[tk];
   }
@@ -108,22 +118,27 @@ mha_bwd_q_kernel(const float* __restrict__ k, const float* __restrict__ v,
   }
 }
 
-// backward B: per key row: dk and dv.
+// backward B: per key row: dk and dv.  DROP: dV sees the dropped weights p * drop.
+template <bool DROP = false>
 __global__ void __launch_bounds__(MHA_THREADS)
 mha_bwd_kv_kernel(const float* __restrict__ q, const float* __restrict__ probs,
                   const float* __restrict__ de, const float* __restrict__ dout,
-                  float* __restrict__ dk, float* __restrict__ dv, int Tq, int Tk, int heads, int dh) {
+                  float* __restrict__ dk, float* __restrict__ dv, int Tq, int Tk, int heads, int dh,
+                  const float* __restrict__ drop) {
   const int tk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int D = heads * dh;
   const float scale = sqrtf((float)dh);
   const float* pcol = probs + ((int64_t)b * heads + h) * Tq * Tk + tk;
   const float* dcol = de + ((int64_t)b * heads + h) * Tq * Tk + tk;
+  const float* rcol = DROP ? drop + ((int64_t)b * heads + h) * Tq * Tk + tk : nullptr;
   for (int d = threadIdx.x; d < dh; d += MHA_THREADS) {
     float ak = 0.f, av = 0.f;
     for (int tq = 0; tq < Tq; ++tq) {
       const int64_t o = ((int64_t)b * Tq + tq) * D + h * dh + d;
       ak = fmaf(dcol[(int64_t)tq * Tk], q[o] / scale, ak);
-      av = fmaf(pcol[(int64_t)tq * Tk], dout[o], av);
+      float p = pcol[(int64_t)tq * Tk];
+      if (DROP) p *= rcol[(int64_t)tq * Tk];
+      av = fmaf(p, dout[o], av);
     }
     const int64_t o = ((int64_t)b * Tk + tk) * D + h * dh + d;
     dk[o] = ak;
@@ -444,14 +459,16 @@ static int mha_fwd_impl(const float* q, const float* k, const float* v, const fl
     NM_LAUNCH_CHECK("nm_mha_fwd(tile)");
     return NM_OK;
   }
-  NM_REQUIRE(!drop, NM_E_UNSUPPORTED, "nm_mha_fwd: attention dropout needs the tiled kernels "
-             "(dh %% 8 == 0, dh <= 128, 8 <= Tq <= 256, Tk <= 256)");
   const size_t smem = sizeof(float) * (size_t)(dh + Tk);
   NM_REQUIRE(smem <= 48 * 1024, NM_E_UNSUPPORTED, "nm_mha_fwd: Tk+dh too large for this kernel");
   dim3 grid((unsigned)Tq, (unsigned)heads, (unsigned)B);
-  mha_fwd_kernel<<<grid, MHA_THREADS, smem, (cudaStream_t)stream>>>(q, k, v, key_mask, causal, out,
-                                                                   probs, (int)Tq, (int)Tk,
-                                                                   (int)heads, (int)dh);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (drop)
+    mha_fwd_kernel<true><<<grid, MHA_THREADS, smem, s>>>(q, k, v, key_mask, causal, out, probs, (int)Tq,
+                                                         (int)Tk, (int)heads, (int)dh, drop);
+  else
+    mha_fwd_kernel<<<grid, MHA_THREADS, smem, s>>>(q, k, v, key_mask, causal, out, probs, (int)Tq, (int)Tk,
+                                                   (int)heads, (int)dh, nullptr);
   NM_LAUNCH_CHECK("nm_mha_fwd");
   return NM_OK;
 }
@@ -514,16 +531,23 @@ static int mha_bwd_impl(const float* q, const float* k, const float* v, const fl
     NM_LAUNCH_CHECK("nm_mha_bwd(kv tile)");
     return NM_OK;
   }
-  NM_REQUIRE(!drop, NM_E_UNSUPPORTED, "nm_mha_bwd: attention dropout needs the tiled kernels");
   const size_t smem = sizeof(float) * (size_t)(dh + Tk);
   NM_REQUIRE(smem <= 48 * 1024, NM_E_UNSUPPORTED, "nm_mha_bwd: Tk+dh too large for this kernel");
   dim3 grid_q((unsigned)Tq, (unsigned)heads, (unsigned)B);
-  mha_bwd_q_kernel<<<grid_q, MHA_THREADS, smem, s>>>(k, v, key_mask, causal, probs, dout, dq, de_work,
-                                                     (int)Tq, (int)Tk, (int)heads, (int)dh);
+  if (drop)
+    mha_bwd_q_kernel<true><<<grid_q, MHA_THREADS, smem, s>>>(k, v, key_mask, causal, probs, dout, dq, de_work,
+                                                             (int)Tq, (int)Tk, (int)heads, (int)dh, drop);
+  else
+    mha_bwd_q_kernel<<<grid_q, MHA_THREADS, smem, s>>>(k, v, key_mask, causal, probs, dout, dq, de_work,
+                                                       (int)Tq, (int)Tk, (int)heads, (int)dh, nullptr);
   NM_LAUNCH_CHECK("nm_mha_bwd(q)");
   dim3 grid_k((unsigned)Tk, (unsigned)heads, (unsigned)B);
-  mha_bwd_kv_kernel<<<grid_k, MHA_THREADS, 0, s>>>(q, probs, de_work, dout, dk, dv, (int)Tq, (int)Tk,
-                                                   (int)heads, (int)dh);
+  if (drop)
+    mha_bwd_kv_kernel<true><<<grid_k, MHA_THREADS, 0, s>>>(q, probs, de_work, dout, dk, dv, (int)Tq, (int)Tk,
+                                                           (int)heads, (int)dh, drop);
+  else
+    mha_bwd_kv_kernel<<<grid_k, MHA_THREADS, 0, s>>>(q, probs, de_work, dout, dk, dv, (int)Tq, (int)Tk,
+                                                     (int)heads, (int)dh, nullptr);
   NM_LAUNCH_CHECK("nm_mha_bwd(kv)");
   return NM_OK;
 }

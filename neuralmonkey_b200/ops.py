@@ -970,7 +970,8 @@ class _MHA(torch.autograd.Function):
 
 
 class _MHADrop(torch.autograd.Function):
-    """_MHA with attention-weight dropout: `drop_mask` [B, heads, Tq, Tk] holds 0 or 1/keep_prob."""
+    """_MHA with attention-weight dropout: `drop_mask` [B, heads, Tq, Tk] holds 0 or 1/keep_prob.  Every
+    shape _MHA takes: both kernel families of csrc/mha.cu apply the mask."""
 
     @staticmethod
     def forward(ctx, q, k, v, key_mask, causal, heads, drop_mask):

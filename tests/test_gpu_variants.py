@@ -117,39 +117,3 @@ def test_var_scopes_through_the_optimizer_kernel():
         assert float(arena.adam_m.abs().sum()) > 0.0
     finally:
         ops.set_gemm_backend("auto")
-
-
-@pytest.mark.parametrize("b,tq,tk,heads,dh,causal", [(2, 9, 9, 4, 8, True), (3, 33, 70, 2, 16, False),
-                                                     (2, 64, 130, 8, 64, False)])
-def test_attention_dropout_in_the_mha_kernels(b, tq, tk, heads, dh, causal):
-    """ops.mha_core with a drop mask (nm_mha_fwd_drop / nm_mha_bwd_drop): context and the gradients of
-    q, k, v against fp64 autograd of softmax(E) * mask . V."""
-    from neuralmonkey_b200 import ops
-    g = torch.Generator().manual_seed(5)
-    d = heads * dh
-    q, k, v = (torch.randn(b, t, d, generator=g) * 0.5 for t in (tq, tk, tk))
-    if causal:
-        k, v = k[:, :tq], v[:, :tq]
-        tk = tq
-    key_mask = (torch.rand(b, tk, generator=g) < 0.8).float()
-    key_mask[:, 0] = 1.0
-    drop = (torch.rand(b, heads, tq, tk, generator=g) < 0.7).float() / 0.7
-    qd, kd, vd = (x.cuda().requires_grad_(True) for x in (q, k, v))
-    out, probs = ops.mha_core(qd, kd, vd, key_mask.cuda(), causal, heads, drop.cuda())
-    dout = torch.randn(b, tq, d, generator=g)
-    out.backward(dout.cuda())
-    q64, k64, v64 = (x.double().requires_grad_(True) for x in (q, k, v))
-
-    def split(x):
-        return x.reshape(b, x.shape[1], heads, dh).transpose(1, 2)
-    e = split(q64) @ split(k64).transpose(-1, -2) / dh ** 0.5
-    if causal:
-        e = torch.where(torch.tril(torch.ones(tq, tk, dtype=torch.bool)), e, torch.full_like(e, -1e9))
-    m = key_mask.double()[:, None, None, :]
-    e = e * m + (1 - m) * -1e9
-    w = torch.softmax(e, -1)
-    ref = ((w * drop.double()) @ split(v64)).transpose(1, 2).reshape(b, tq, d)
-    ref.backward(dout.double())
-    assert max_abs(out, ref) < 1e-4 and max_abs(probs, w) < 1e-5
-    for got, ref_grad in ((qd.grad, q64.grad), (kd.grad, k64.grad), (vd.grad, v64.grad)):
-        assert float((got.cpu().double() - ref_grad).norm()) <= 1e-4 * float(ref_grad.norm()) + 1e-7
