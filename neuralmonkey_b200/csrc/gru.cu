@@ -178,12 +178,14 @@ ClusterPlan plan_clusters(int64_t B, int64_t H, int sm_budget, bool backward) {
   int max_clusters = resident_clusters(backward);
   if (sm_budget > 0 && sm_budget / GC_CLUSTER < max_clusters) max_clusters = sm_budget / GC_CLUSTER;
   if (max_clusters < 1) max_clusters = 1;
+  // The kernels walk their rows GC_RB at a time, so Bc only needs to be a multiple of GC_RB: rounding it
+  // further (to 4, say) would take B = 256 on 15 clusters from 18 rows to 20, leaving two clusters idle.
   int Bc = (int)((B + max_clusters - 1) / max_clusters);
-  Bc = (Bc + 3) / 4 * 4;
+  Bc = (Bc + GC_RB - 1) / GC_RB * GC_RB;
   const size_t per_row = (size_t)(backward ? gc_bwd_row_floats(p.sl) : gc_fwd_row_floats(p.sl)) * 4;
-  const int cap = (int)((GC_SMEM_CAP - GC_BAR_BYTES) / per_row) / 4 * 4;
+  const int cap = (int)((GC_SMEM_CAP - GC_BAR_BYTES) / per_row) / GC_RB * GC_RB;
   if (Bc > cap) Bc = cap;
-  if (Bc < 4) Bc = 4;
+  if (Bc < GC_RB) Bc = GC_RB;
   p.Bc = Bc;
   p.nclusters = (int)((B + Bc - 1) / Bc);
   p.smem = GC_BAR_BYTES + per_row * Bc;
