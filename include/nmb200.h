@@ -7,7 +7,7 @@
  * (neuralmonkey/tf_manager.py:179-180).  Every entry point below replaces the
  * TF op group named in its comment (reference file:line), and is what a
  * ctypes binding inside the reference's ModelPart classes would call
- * (see INTEGRATION.md).
+ * (see INTEGRATION.md).  73 entry points.
  *
  * Conventions
  *   - plain pointers + int64_t sizes; no torch / C++ types cross the ABI;
@@ -347,6 +347,16 @@ int nm_clip_adam_step(float* params, float* grads, float* m, float* v,
                                                with the schedule's next value */,
                       void* stream);
 
+/* tf.train.AdadeltaOptimizer (trainers/generic_trainer.py:172-190 with an Adadelta optimizer, tests/str.ini) after
+ * the same regularisation and per-tensor clip_by_norm as nm_clip_adam_step, over the same arena and segment tables:
+ *   accum = rho*accum + (1-rho)*g^2;  update = sqrt(accum_update + eps) / sqrt(accum + eps) * g;
+ *   accum_update = rho*accum_update + (1-rho)*update^2;  p -= lr*update
+ * Segments flagged lazy (bit 1) skip entries whose gradient is exactly zero.  lr_dev: as lr_t_dev above. */
+int nm_clip_adadelta_step(float* params, float* grads, float* accum, float* accum_update, const int64_t* seg_off,
+                          const uint8_t* seg_reg, float* norms, int64_t n, int64_t nseg, float grad_scale,
+                          const float* grad_denominator, float lr, float rho, float eps, float clip_norm, float l1,
+                          float l2, float* l1l2_out, const float* lr_dev, void* stream);
+
 /* ---- K8: multi-head scaled dot-product attention core ---------------------------
  * Replaces attention() of attention/scaled_dot_product.py:98-226 between the
  * q/k/v projections and the output projection:
@@ -409,6 +419,54 @@ int nm_im2col3x3(const float* x, float* cols, int64_t N, int64_t H, int64_t W,
 /* 2x2 / stride 2 max pool, NHWC (H, W even). */
 int nm_maxpool2x2_fwd(const float* x, float* y, int64_t N, int64_t H, int64_t W,
                       int64_t C, void* stream);
+
+/* ---- K12b: trainable CNN layers (encoders/cnn_encoder.py:209-320: tf.layers.conv2d, batch_normalization,
+ * max_pooling2d / average_pooling2d) --------------------------------------------------------------------------
+ * NHWC fp32, filters HWIO.  Convolutions have stride 1 (the reference never strides them).
+ *
+ * nm_conv2d_fwd: y [N,Ho,Wo,Cout] = act(conv(x [N,H,W,Cin], w) + bias), Ho = H + pad_top + pad_bottom - k + 1
+ * (Wo likewise); `same` in TF's convention is pad_top = (k-1)/2, pad_bottom = k-1-pad_top, `valid` all zero.
+ * w is [k,k,Cin,Cout]; with flip = 1 it is [k,k,Cout,Cin] and is applied turned by 180 degrees with its channel
+ * axes swapped: the data gradient of a forward convolution with pads (t, b, l, r) is this call on dY with
+ * pads (k-1-t, k-1-b, k-1-l, k-1-r), flip = 1, no bias.  bias may be NULL; act is NM_ACT_NONE or NM_ACT_RELU.
+ * An implicit GEMM (no patch matrix): backend NM_GEMM_SIMT = exact fp32 on the CUDA cores, NM_GEMM_AUTO /
+ * NM_GEMM_TC = wgmma with TF32 operands.
+ * nm_conv2d_wgrad: dw [k,k,Cin,Cout] += sum over the output pixels of patch(x)^T dy, db [Cout] += sum dy (db may
+ * be NULL).  The pixel reduction is split over CTAs into `workspace` (>= (k*k*Cin+1)*Cout floats; more lets it
+ * split further) and the partials are added in a fixed order: two calls give identical bits.
+ * nm_conv2d_wgrad_workspace: the workspace (floats) at which nm_conv2d_wgrad splits as far as it wants to for that
+ * shape and backend, or -1 for invalid sizes. */
+int nm_conv2d_fwd(const float* x, const float* w, const float* bias, float* y, int64_t N, int64_t H, int64_t W,
+                  int64_t Cin, int64_t Cout, int64_t k, int64_t pad_top, int64_t pad_bottom, int64_t pad_left,
+                  int64_t pad_right, int flip, int act, int backend, void* stream);
+int64_t nm_conv2d_wgrad_workspace(int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout, int64_t k,
+                                  int64_t pad_top, int64_t pad_bottom, int64_t pad_left, int64_t pad_right,
+                                  int backend);
+int nm_conv2d_wgrad(const float* x, const float* dy, float* dw, float* db, float* workspace, int64_t workspace_floats,
+                    int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout, int64_t k, int64_t pad_top,
+                    int64_t pad_bottom, int64_t pad_left, int64_t pad_right, int backend, void* stream);
+/* tf.layers.batch_normalization over the P = N*H*W rows of x [P,C] (+ the ReLU after it when relu = 1):
+ * y = gamma * (x - mean) * invstd + beta, invstd = 1/sqrt(var + eps).  training = 1: mean and the biased var of the
+ * batch (sums in fp64), and in the same call moving = momentum*moving + (1-momentum)*batch value, with the
+ * Bessel-corrected batch variance for moving_var (TF 1.x fused batch norm); training = 0: the moving statistics.
+ * save_mean / save_invstd [C] receive what was used.  workspace: NM_BN_WS_DOUBLES_PER_CHANNEL * C doubles (may
+ * be NULL when training = 0).  Backward: dx (may be NULL) and dgamma, dbeta += (may be NULL), summed in a fixed
+ * order. */
+#define NM_BN_WS_DOUBLES_PER_CHANNEL 130
+int nm_batchnorm_fwd(const float* x, const float* gamma, const float* beta, float* y, float* moving_mean,
+                     float* moving_var, float* save_mean, float* save_invstd, double* workspace, int64_t P, int64_t C,
+                     float momentum, float eps, int training, int relu, void* stream);
+int nm_batchnorm_bwd(const float* x, const float* dy, const float* gamma, const float* beta, const float* save_mean,
+                     const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* workspace, int64_t P,
+                     int64_t C, int training, int relu, void* stream);
+/* k x k pooling with stride `stride`, max (is_max = 1) or average, NHWC.  same = 0: `valid`, Ho = (H-k)/stride+1;
+ * same = 1: Ho = ceil(H/stride), padded TF's way (odd pixel at the bottom / right), averages over the pixels inside
+ * the image.  The backward pass writes dx [N,H,W,C] (x is only read for max pooling); max pooling routes each
+ * window's gradient to its first maximal pixel in row-major order, as TF does. */
+int nm_pool2d_fwd(const float* x, float* y, int64_t N, int64_t H, int64_t W, int64_t C, int64_t k, int64_t stride,
+                  int same, int is_max, void* stream);
+int nm_pool2d_bwd(const float* x, const float* dy, float* dx, int64_t N, int64_t H, int64_t W, int64_t C, int64_t k,
+                  int64_t stride, int same, int is_max, void* stream);
 
 /* ---- gate arithmetic of the step-wise cell variants (SURVEY.md 8(f) N4) ------------------------------
  * NematusGRUCell (nn/ortho_gru_cell.py:57-105) after its four projections: sg = state_proj_g(state) [B,2H],

@@ -146,6 +146,37 @@ clip_adam_kernel(float* __restrict__ params, const float* __restrict__ grads, fl
   }
 }
 
+
+// tf.train.AdadeltaOptimizer after the same clip_by_norm as clip_adam_kernel:
+//   accum = rho*accum + (1-rho)*g^2;  update = sqrt(accum_update + eps) / sqrt(accum + eps) * g;
+//   accum_update = rho*accum_update + (1-rho)*update^2;  p -= lr*update
+__global__ void __launch_bounds__(OPT_THREADS)
+clip_adadelta_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ accum,
+                     float* __restrict__ accum_update, const int64_t* __restrict__ seg_off,
+                     const uint8_t* __restrict__ seg_reg, const float* __restrict__ norms, int64_t n, int64_t nseg, float lr, float rho, float eps,
+                     float clip_norm, const float* __restrict__ lr_dev) {
+  if (lr_dev) lr = lr_dev[0];
+  const int64_t c0 = (int64_t)blockIdx.x * OPT_CHUNK;
+  const int64_t c1 = min(n, c0 + OPT_CHUNK);
+  int64_t seg = find_segment(seg_off, nseg, c0);
+  while (seg < nseg && seg_off[seg] < c1) {
+    const int64_t a = max(c0, seg_off[seg]), b = min(c1, seg_off[seg + 1]);
+    const float scale = clip_norm > 0.f ? clip_norm / fmaxf(sqrtf(norms[seg]), clip_norm) : 1.f;
+    const bool lazy = (seg_reg[seg] & 2) != 0;     // (segments outside a trainer's var_scopes)
+#pragma unroll 1
+    for (int64_t i = a + threadIdx.x; i < b; i += OPT_THREADS) {
+      const float g = grads[i] * scale;
+      if (lazy && g == 0.f) continue;
+      const float acc = rho * accum[i] + (1.f - rho) * g * g;
+      const float upd = sqrtf(accum_update[i] + eps) / sqrtf(acc + eps) * g;
+      accum[i] = acc;
+      accum_update[i] = rho * accum_update[i] + (1.f - rho) * upd * upd;
+      params[i] -= lr * upd;
+    }
+    ++seg;
+  }
+}
+
 }  // namespace nm
 
 using namespace nm;
@@ -174,6 +205,31 @@ int nm_clip_adam_step(float* params, float* grads, float* m, float* v, const int
   clip_adam_kernel<<<blocks, OPT_THREADS, 0, s>>>(params, grads, m, v, seg_off, seg_reg, norms, n, nseg, lr_t,
                                                   beta1, beta2, eps, clip_norm, lr_t_dev);
   NM_LAUNCH_CHECK("nm_clip_adam_step(adam)");
+  return NM_OK;
+}
+
+int nm_clip_adadelta_step(float* params, float* grads, float* accum, float* accum_update, const int64_t* seg_off,
+                          const uint8_t* seg_reg, float* norms, int64_t n, int64_t nseg, float grad_scale,
+                          const float* grad_denominator, float lr, float rho, float eps, float clip_norm, float l1,
+                          float l2, float* l1l2_out, const float* lr_dev, void* stream) {
+  NM_REQUIRE(params && grads && accum && accum_update && seg_off && seg_reg && norms, NM_E_INVALID,
+             "nm_clip_adadelta_step: null pointer");
+  NM_REQUIRE(n > 0 && nseg > 0, NM_E_INVALID, "nm_clip_adadelta_step: bad sizes");
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned blocks = (unsigned)ceil_div(n, OPT_CHUNK);
+  const bool need_pass1 =
+      clip_norm > 0.f || l1 != 0.f || l2 != 0.f || grad_scale != 1.f || grad_denominator != nullptr ||
+      l1l2_out != nullptr;
+  if (need_pass1) {
+    NM_CUDA_TRY(cudaMemsetAsync(norms, 0, sizeof(float) * nseg, s));
+    if (l1l2_out) NM_CUDA_TRY(cudaMemsetAsync(l1l2_out, 0, sizeof(float) * 2, s));
+    reg_norm_kernel<<<blocks, OPT_THREADS, 0, s>>>(params, grads, seg_off, seg_reg, norms, n, nseg,
+                                                   grad_scale, grad_denominator, l1, l2, l1l2_out);
+    NM_LAUNCH_CHECK("nm_clip_adadelta_step(reg_norm)");
+  }
+  clip_adadelta_kernel<<<blocks, OPT_THREADS, 0, s>>>(params, grads, accum, accum_update, seg_off, seg_reg, norms, n, nseg, lr,
+                                                      rho, eps, clip_norm, lr_dev);
+  NM_LAUNCH_CHECK("nm_clip_adadelta_step(adadelta)");
   return NM_OK;
 }
 

@@ -1258,3 +1258,174 @@ def maxpool2x2(x: torch.Tensor) -> torch.Tensor:
     y = torch.empty(n, h // 2, wd // 2, c, device=x.device, dtype=torch.float32)
     call("nm_maxpool2x2_fwd", ptr(x), ptr(y), n, h, wd, c, lib.stream())
     return y
+
+
+# ---------------------------------------------------------------------------
+# K12b trainable CNN layers (encoders/cnn_encoder.py): convolution, batch normalization, pooling
+# ---------------------------------------------------------------------------
+def conv_pads(k: int, padding: str) -> Tuple[int, int]:
+    """(before, after) of one spatial axis at stride 1: TensorFlow's `same` puts the odd pixel after."""
+    if padding == "valid":
+        return 0, 0
+    if padding == "same":
+        return (k - 1) // 2, k - 1 - (k - 1) // 2
+    raise ValueError("padding must be 'same' or 'valid', got {!r}".format(padding))
+
+
+def _conv_backend() -> int:
+    """The exact fp32 kernels under the 'simt' GEMM backend, wgmma with TF32 operands otherwise."""
+    return lib.GEMM_SIMT if _GEMM_BACKEND == lib.GEMM_SIMT else lib.GEMM_AUTO
+
+
+# the weight-gradient partials of one call: as many [k*k*Cin+1, Cout] slices as the kernel splits the pixel
+# reduction into (nm_conv2d_wgrad_workspace), at most 64 MB, at least one slice
+_WGRAD_WS_FLOATS = 16 << 20
+
+
+def conv_wgrad_workspace(n, h, wd, cin, cout, k, pt, pb, backend) -> int:
+    want = int(lib.load().nm_conv2d_wgrad_workspace(n, h, wd, cin, cout, k, pt, pb, pt, pb, backend))
+    if want < 0:
+        raise ValueError("conv2d: bad sizes {}".format((n, h, wd, cin, cout, k, pt, pb)))
+    return max((k * k * cin + 1) * cout, min(_WGRAD_WS_FLOATS, want))
+
+
+class _Conv2d(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b, padding, act):
+        n, h, wd, cin = x.shape
+        k, cout = w.shape[0], w.shape[3]
+        if w.shape[1] != k or w.shape[2] != cin:
+            raise ValueError("conv2d: filter {} does not fit input {}".format(tuple(w.shape), tuple(x.shape)))
+        pt, pb = conv_pads(k, padding)
+        x = _f32(x).contiguous()
+        w = _f32(w).contiguous()
+        ho, wo = h + pt + pb - k + 1, wd + pt + pb - k + 1
+        y = torch.empty(n, ho, wo, cout, device=x.device, dtype=torch.float32)
+        backend = _conv_backend()
+        call("nm_conv2d_fwd", ptr(x), ptr(w), ptr(b), ptr(y), n, h, wd, cin, cout, k, pt, pb, pt, pb, 0,
+             lib.NM_ACT[act], backend, lib.stream())
+        ctx.save_for_backward(x, w, y if act is not None else None)
+        ctx.geom = (n, h, wd, cin, cout, k, pt, pb, backend, act)
+        ctx.sinks = (_sink(w), _sink(b) if b is not None else None)
+        ctx.has_bias = b is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, y = ctx.saved_tensors
+        n, h, wd, cin, cout, k, pt, pb, backend, act = ctx.geom
+        dy = dy.contiguous()
+        if act is not None:
+            dpre = torch.empty_like(dy)
+            call("nm_act_bwd", ptr(y), ptr(dy), ptr(dpre), dy.numel(), lib.NM_ACT[act], lib.stream())
+            dy = dpre
+        ho, wo = dy.shape[1], dy.shape[2]
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            call("nm_conv2d_fwd", ptr(dy), ptr(w), None, ptr(dx), n, ho, wo, cout, cin, k, k - 1 - pt, k - 1 - pb,
+                 k - 1 - pt, k - 1 - pb, 1, 0, backend, lib.stream())
+        w_sink, b_sink = ctx.sinks
+        dw = w_sink if w_sink is not None else torch.zeros_like(w)
+        db = None
+        if ctx.has_bias:
+            db = b_sink if b_sink is not None else torch.zeros(cout, device=x.device, dtype=torch.float32)
+        ws = torch.empty(conv_wgrad_workspace(n, h, wd, cin, cout, k, pt, pb, backend), device=x.device,
+                         dtype=torch.float32)
+        call("nm_conv2d_wgrad", ptr(x), ptr(dy), ptr(dw), ptr(db), ptr(ws), ws.numel(), n, h, wd, cin, cout, k, pt,
+             pb, pt, pb, backend, lib.stream())
+        return (dx, None if w_sink is not None else dw,
+                None if (b_sink is not None or not ctx.has_bias) else db, None, None)
+
+
+def conv2d(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], padding: str,
+           act: Optional[str] = None) -> torch.Tensor:
+    """tf.layers.conv2d at stride 1: NHWC x, HWIO w, `same` or `valid` padding, act None or 'relu'."""
+    if act not in (None, "relu"):
+        raise ValueError("conv2d: act must be None or 'relu'")
+    return _Conv2d.apply(x, w, b, padding, act)
+
+
+BN_WS_DOUBLES_PER_CHANNEL = 130     # NM_BN_WS_DOUBLES_PER_CHANNEL
+
+
+class _BatchNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, gamma, beta, moving_mean, moving_var, training, relu, momentum, eps):
+        c = x.shape[-1]
+        x2 = _f32(x).contiguous()
+        p = x2.numel() // c
+        y = torch.empty_like(x2)
+        mean = torch.empty(c, device=x.device, dtype=torch.float32)
+        invstd = torch.empty(c, device=x.device, dtype=torch.float32)
+        ws = torch.empty(BN_WS_DOUBLES_PER_CHANNEL * c, device=x.device, dtype=torch.float64)
+        call("nm_batchnorm_fwd", ptr(x2), ptr(gamma), ptr(beta), ptr(y), ptr(moving_mean), ptr(moving_var), ptr(mean),
+             ptr(invstd), ptr(ws), p, c, float(momentum), float(eps), int(training), int(relu), lib.stream())
+        ctx.save_for_backward(x2, gamma, beta, mean, invstd)
+        ctx.flags = (int(training), int(relu))
+        ctx.sinks = (_sink(gamma), _sink(beta))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x2, gamma, beta, mean, invstd = ctx.saved_tensors
+        training, relu = ctx.flags
+        c = x2.shape[-1]
+        p = x2.numel() // c
+        dy = dy.contiguous()
+        dx = torch.empty_like(x2)
+        sg, sb = ctx.sinks
+        dg = sg if sg is not None else torch.zeros(c, device=dy.device, dtype=torch.float32)
+        db = sb if sb is not None else torch.zeros(c, device=dy.device, dtype=torch.float32)
+        ws = torch.empty(BN_WS_DOUBLES_PER_CHANNEL * c, device=dy.device, dtype=torch.float64)
+        call("nm_batchnorm_bwd", ptr(x2), ptr(dy), ptr(gamma), ptr(beta), ptr(mean), ptr(invstd), ptr(dx), ptr(dg),
+             ptr(db), ptr(ws), p, c, training, relu, lib.stream())
+        return (dx, None if sg is not None else dg, None if sb is not None else db,
+                None, None, None, None, None, None)
+
+
+def batch_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, moving_mean: torch.Tensor,
+               moving_var: torch.Tensor, training: bool, relu: bool = False, momentum: float = 0.99,
+               eps: float = 1e-3) -> torch.Tensor:
+    """tf.layers.batch_normalization over the last axis (TF 1.x defaults), optionally followed by ReLU.  In
+    training the moving statistics are updated in place (the UPDATE_OPS the reference's trainer runs)."""
+    return _BatchNorm.apply(x, gamma, beta, moving_mean, moving_var, bool(training), bool(relu), momentum, eps)
+
+
+def pool_out(size: int, k: int, stride: int, padding: str) -> int:
+    if padding == "same":
+        return -(-size // stride)
+    return (size - k) // stride + 1
+
+
+class _Pool2d(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, k, stride, padding, is_max):
+        n, h, wd, c = x.shape
+        x = _f32(x).contiguous()
+        y = torch.empty(n, pool_out(h, k, stride, padding), pool_out(wd, k, stride, padding), c, device=x.device,
+                        dtype=torch.float32)
+        same = int(padding == "same")
+        call("nm_pool2d_fwd", ptr(x), ptr(y), n, h, wd, c, k, stride, same, int(is_max), lib.stream())
+        ctx.save_for_backward(x)
+        ctx.geom = (k, stride, same, int(is_max))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        k, stride, same, is_max = ctx.geom
+        n, h, wd, c = x.shape
+        dx = torch.empty_like(x)
+        call("nm_pool2d_bwd", ptr(x), ptr(dy.contiguous()), ptr(dx), n, h, wd, c, k, stride, same, is_max,
+             lib.stream())
+        return dx, None, None, None, None
+
+
+def pool2d(x: torch.Tensor, k: int, stride: int, padding: str, kind: str) -> torch.Tensor:
+    """tf.layers.max_pooling2d (kind 'max') / average_pooling2d ('avg') over NHWC x."""
+    if padding not in ("same", "valid"):
+        raise ValueError("padding must be 'same' or 'valid', got {!r}".format(padding))
+    if kind not in ("max", "avg"):
+        raise ValueError("pooling kind must be 'max' or 'avg'")
+    return _Pool2d.apply(x, int(k), int(stride), padding, kind == "max")

@@ -42,6 +42,16 @@ class LazyAdamOptimizer(Optimizer):
     lazy = True
 
 
+class AdadeltaOptimizer(Optimizer):
+    """tf.train.AdadeltaOptimizer; the update is nm_clip_adadelta_step (the two accumulators take the two
+    optimizer slots of the arena)."""
+
+    def __init__(self, learning_rate=0.001, rho: float = 0.95, epsilon: float = 1e-8, use_locking: bool = False,
+                 name: str = "Adadelta") -> None:
+        Optimizer.__init__(self, learning_rate, epsilon=epsilon, use_locking=use_locking, name=name)
+        self.rho = rho
+
+
 def random_uniform_initializer(minval=0.0, maxval=1.0, seed=None, dtype=None):
     return uniform_initializer(minval, maxval)
 
@@ -60,7 +70,7 @@ def variance_scaling_initializer(scale=1.0, mode="fan_in", distribution="normal"
     return _vs(scale=scale, mode=mode, distribution=dist)
 
 
-train = SimpleNamespace(AdamOptimizer=AdamOptimizer, Optimizer=Optimizer)
+train = SimpleNamespace(AdamOptimizer=AdamOptimizer, AdadeltaOptimizer=AdadeltaOptimizer, Optimizer=Optimizer)
 contrib = SimpleNamespace(opt=SimpleNamespace(LazyAdamOptimizer=LazyAdamOptimizer))
 tanh = "tanh"
 sigmoid = "sigmoid"

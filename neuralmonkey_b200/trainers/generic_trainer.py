@@ -5,6 +5,7 @@ One `train_step()` =
     -> backward of the objectives (weight gradients accumulate straight into the arena)
     -> [data parallel: one all-reduce of gradients + loss sum + token count]
     -> nm_clip_adam_step: L1/L2 terms, per-tensor clip_by_norm, TF-Adam (K13)
+       (nm_clip_adadelta_step for tf.train.AdadeltaOptimizer)
 with no device->host synchronisation inside; the losses are returned as device tensors.
 """
 import math
@@ -397,6 +398,8 @@ class GenericTrainer(GraphExecutor, Feedable):
         opt.steps += 1
         t = opt.steps
         lr = opt.lr_at(self.global_step - 1)
+        if isinstance(opt, tf.AdadeltaOptimizer):
+            return lr
         return lr * math.sqrt(1.0 - opt.beta2 ** t) / (1.0 - opt.beta1 ** t)
 
     def apply_gradients(self, grad_scale: float = 1.0,
@@ -423,8 +426,15 @@ class GenericTrainer(GraphExecutor, Feedable):
         if self.var_scopes is not None:
             seg_flags, mask = self._scope_restriction(seg_flags)
             arena.grads.mul_(mask)
+        clip = float(self.clip_norm) if self.clip_norm else 0.0
+        if isinstance(opt, tf.AdadeltaOptimizer):
+            call("nm_clip_adadelta_step", ptr(arena.params), ptr(arena.grads), ptr(adam_m), ptr(adam_v),
+                 ptr(arena.seg_off), ptr(seg_flags), ptr(arena.seg_norms), n, len(arena.train_names),
+                 float(grad_scale), ptr(denominator), float(lr_t), float(opt.rho), float(opt.epsilon), clip,
+                 float(self.l1_weight), float(self.l2_weight), ptr(self._l1l2_buf), ptr(lr_t_dev), lib.stream())
+            return
         common = (float(opt.beta1), float(opt.beta2), float(opt.epsilon),
-                  float(self.clip_norm) if self.clip_norm else 0.0, float(self.l1_weight), float(self.l2_weight))
+                  clip, float(self.l1_weight), float(self.l2_weight))
         call("nm_clip_adam_step", ptr(arena.params), ptr(arena.grads), ptr(adam_m),
              ptr(adam_v), ptr(arena.seg_off), ptr(seg_flags), ptr(arena.seg_norms), n,
              len(arena.train_names), float(grad_scale), ptr(denominator), float(lr_t), *common,
