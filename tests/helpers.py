@@ -8,12 +8,14 @@ from oracle import nm_oracle as O
 
 
 def build_bahdanau(vs=60, vt=70, es=11, he=7, et=9, hd=8, out=9, maxout=True, max_len=10,
-                   supress_unk=True, l1=0.0, l2=0.0, clip=None, lr=1e-4, cuda_graph=False):
-    """Encoder + attention + decoder + trainer of tests/bahdanau.ini's shape family."""
+                   supress_unk=True, l1=0.0, l2=0.0, clip=None, lr=1e-4, cuda_graph=False, out_act=None):
+    """Encoder + attention + decoder + trainer of tests/bahdanau.ini's shape family.  Without maxout, `out_act`
+    ("tanh", "relu" or "sigmoid") selects a dense output projection of size `out` with that activation;
+    None keeps the decoder's default."""
     from neuralmonkey_b200 import runtime
     from neuralmonkey_b200.attention import Attention
     from neuralmonkey_b200.decoders import Decoder
-    from neuralmonkey_b200.decoders.output_projection import maxout_output
+    from neuralmonkey_b200.decoders.output_projection import maxout_output, nonlinear_output
     from neuralmonkey_b200.encoders import SentenceEncoder
     from neuralmonkey_b200.trainers import CrossEntropyTrainer
     from neuralmonkey_b200 import tf
@@ -27,7 +29,8 @@ def build_bahdanau(vs=60, vt=70, es=11, he=7, et=9, hd=8, out=9, maxout=True, ma
     att = Attention(name="attention", encoder=enc)
     dec = Decoder(encoders=[enc], vocabulary=tgt_vocab, data_id="target", name="decoder",
                   max_output_len=max_len, rnn_size=hd, embedding_size=et, attentions=[att],
-                  output_projection=maxout_output(out) if maxout else None,
+                  output_projection=(maxout_output(out) if maxout else
+                                     nonlinear_output(out, out_act) if out_act else None),
                   supress_unk=supress_unk)
     trainer = CrossEntropyTrainer(decoders=[dec], l1_weight=l1, l2_weight=l2, clip_norm=clip,
                                   optimizer=tf.AdamOptimizer(learning_rate=lr), use_cuda_graph=cuda_graph)

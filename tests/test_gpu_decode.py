@@ -16,8 +16,12 @@ MID = dict(vs=120, vt=200, es=32, he=16, et=32, hd=32, out=32, maxout=False, max
            supress_unk=False)
 
 
-def _step_reference(p, symbols, h_prev, parent, group):
-    """fp64 restatement of one step for rows [rows]; p: dict of fp32 CPU tensors."""
+ACT_FN = {"none": lambda z: z, "tanh": torch.tanh, "relu": torch.relu, "sigmoid": torch.sigmoid}
+
+
+def _step_reference(p, symbols, h_prev, parent, group, act="tanh"):
+    """fp64 restatement of one step for rows [rows]; p: dict of fp32 CPU tensors.  `act` is the activation of
+    a dense output projection (ignored with maxout)."""
     d = {k: (v.double() if torch.is_tensor(v) and v.dtype == torch.float32 else v) for k, v in p.items()}
     rows = symbols.shape[0]
     x = d["table"][symbols]
@@ -44,22 +48,13 @@ def _step_reference(p, symbols, h_prev, parent, group):
         o = z.shape[1] // 2
         out = torch.maximum(z[:, :o], z[:, o:])
     else:
-        out = torch.tanh(z)
+        out = ACT_FN[act](z)
     return hn, ctx, w, out
 
 
-@pytest.mark.parametrize("cluster", ["", "1", "2", "4", "8"])
-@pytest.mark.parametrize("dims", [
-    # rows, group, E, H, A, C, Tx, O, maxout, masked
-    (5, 1, 9, 8, 14, 14, 7, 9, True, True),            # tests/bahdanau.ini dims: scalar variant
-    (21, 1, 32, 32, 64, 48, 13, 32, False, True),      # 16-byte rows: TMA-staged tiles, ragged last cluster
-    (24, 3, 32, 40, 64, 64, 50, 32, True, False),      # beam rows sharing an encoder row, no mask
-    (64, 8, 300, 300, 600, 600, 50, 300, False, True),  # en-de dims, beam 8
-])
-def test_step_kernel_against_fp64(monkeypatch, dims, cluster):
-    from neuralmonkey_b200 import lib
-    rows, group, e, h, a, c, tx, o, maxout, masked = dims
-    monkeypatch.setenv("NMB200_DECSTEP_CLUSTER", cluster)
+def _step_inputs(dims):
+    """Random parameters, symbols, previous states and parents of one step (fp32 CPU tensors)."""
+    rows, group, e, h, a, c, tx, o, maxout, masked = dims[:10]
     g = torch.Generator().manual_seed(rows * 7 + tx)
     vocab, nb = 50, rows // group
 
@@ -77,28 +72,92 @@ def test_step_kernel_against_fp64(monkeypatch, dims, cluster):
     symbols = torch.randint(0, vocab, (rows,), generator=g)
     h_prev = rnd(rows, h, scale=0.5)
     parent = torch.randint(0, group, (rows,), generator=g).int() if group > 1 else None
-    want = _step_reference(p, symbols, h_prev, parent, group)
+    return p, symbols, h_prev, parent
+
+
+def _run_step(dims, p, symbols, h_prev, parent, act="tanh", x_in=None, outputs=("x", "ctx", "w")):
+    """One nm_attn_decoder_step_fwd launch; symbols go through the table unless x_in [rows, E] is given.  The
+    optional outputs not named in `outputs` are passed as NULL.  Returns {name: CUDA tensor}."""
+    from neuralmonkey_b200 import lib
+    rows, group, e, h, a, c, tx, o, maxout, masked = dims[:10]
     dv = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in p.items()}
-    out_h = torch.empty(rows, h, device="cuda")
-    out_ctx = torch.empty(rows, c, device="cuda")
-    out_w = torch.empty(rows, tx, device="cuda")
-    out = torch.empty(rows, o, device="cuda")
-    x_out = torch.empty(rows, e, device="cuda")
+    res = {"h": torch.full((rows, h), float("nan"), device="cuda"),
+           "out": torch.full((rows, o), float("nan"), device="cuda")}
+    for name, width in (("x", e), ("ctx", c), ("w", tx)):
+        if name in outputs:
+            res[name] = torch.full((rows, width), float("nan"), device="cuda")
+    # held in variables until the launch has run: the kernel only gets their raw pointers
     sym_d, hp_d = symbols.cuda(), h_prev.cuda()
+    x_d = x_in.cuda() if x_in is not None else None
     par_d = parent.cuda() if parent is not None else None
-    lib.call("nm_attn_decoder_step_fwd", lib.ptr(sym_d), lib.ptr(dv["table"]), None, lib.ptr(hp_d), lib.ptr(par_d),
+    lib.call("nm_attn_decoder_step_fwd", lib.ptr(sym_d), lib.ptr(dv["table"]), lib.ptr(x_d), lib.ptr(hp_d),
+             lib.ptr(par_d),
              lib.ptr(dv["wg"]), lib.ptr(dv["bg"]), lib.ptr(dv["wc"]), lib.ptr(dv["bc"]), lib.ptr(dv["wq"]),
              lib.ptr(dv["bq"]), lib.ptr(dv["v"]), lib.ptr(dv["ab"]), lib.ptr(dv["keys"]), lib.ptr(dv["values"]),
-             lib.ptr(dv["mask"]), lib.ptr(dv["wo"]), lib.ptr(dv["bo"]), lib.ptr(x_out), lib.ptr(out_h),
-             lib.ptr(out_ctx), lib.ptr(out_w), lib.ptr(out), rows, group, e, h, a, c, tx, o, 1, int(maxout),
-             lib.stream())
+             lib.ptr(dv["mask"]), lib.ptr(dv["wo"]), lib.ptr(dv["bo"]), lib.ptr(res.get("x")), lib.ptr(res["h"]),
+             lib.ptr(res.get("ctx")), lib.ptr(res.get("w")), lib.ptr(res["out"]), rows, group, e, h, a, c, tx, o,
+             lib.NM_ACT[act], int(maxout), lib.stream())
     torch.cuda.synchronize()
-    assert torch.equal(x_out.cpu(), p["table"][symbols])
+    return res
+
+
+@pytest.mark.parametrize("cluster", ["", "1", "2", "4", "8"])
+@pytest.mark.parametrize("dims", [
+    # rows, group, E, H, A, C, Tx, O, maxout, masked, act of a dense output
+    (5, 1, 9, 8, 14, 14, 7, 9, True, True, "tanh"),            # tests/bahdanau.ini dims: scalar variant
+    (21, 1, 32, 32, 64, 48, 13, 32, False, True, "tanh"),      # 16-byte rows: TMA-staged tiles, ragged last cluster
+    (24, 3, 32, 40, 64, 64, 50, 32, True, False, "tanh"),      # beam rows sharing an encoder row, no mask
+    (64, 8, 300, 300, 600, 600, 50, 300, False, True, "tanh"),  # en-de dims, beam 8
+    # every other activation of a dense output projection
+    (21, 1, 32, 32, 64, 48, 13, 32, False, True, "none"),
+    (21, 1, 32, 32, 64, 48, 13, 32, False, True, "relu"),
+    (21, 1, 32, 32, 64, 48, 13, 32, False, True, "sigmoid"),
+    (64, 8, 300, 300, 600, 600, 50, 300, False, True, "none"),
+    (64, 8, 300, 300, 600, 600, 50, 300, False, True, "relu"),
+    (64, 8, 300, 300, 600, 600, 50, 300, False, True, "sigmoid"),
+    # scalar variant with beam rows and a parent gather, both output kinds
+    (12, 3, 9, 8, 14, 14, 7, 9, True, True, "tanh"),
+    (12, 3, 9, 8, 14, 14, 7, 9, False, False, "relu"),
+])
+def test_step_kernel_against_fp64(monkeypatch, dims, cluster):
+    act = dims[10]
+    monkeypatch.setenv("NMB200_DECSTEP_CLUSTER", cluster)
+    p, symbols, h_prev, parent = _step_inputs(dims)
+    want = _step_reference(p, symbols, h_prev, parent, dims[1], act)
+    got = _run_step(dims, p, symbols, h_prev, parent, act)
+    assert torch.equal(got["x"].cpu(), p["table"][symbols])
     tol = 3e-5
-    assert max_abs(out_h, want[0]) < tol
-    assert max_abs(out_w, want[2]) < tol
-    assert max_abs(out_ctx, want[1]) < tol
-    assert max_abs(out, want[3]) < tol
+    assert max_abs(got["h"], want[0]) < tol
+    assert max_abs(got["w"], want[2]) < tol
+    assert max_abs(got["ctx"], want[1]) < tol
+    assert max_abs(got["out"], want[3]) < tol
+
+
+STEP_DIMS = [(21, 1, 32, 32, 64, 48, 13, 32, False, True),    # vector variant
+             (12, 3, 9, 8, 14, 14, 7, 9, True, True)]         # scalar variant, parent gather
+
+
+@pytest.mark.parametrize("dims", STEP_DIMS)
+def test_step_kernel_x_in_equals_the_table_path(dims):
+    """Already-embedded inputs (x_in) give bit for bit the step fed through the table; `symbols` is then
+    ignored, so other (valid) ids may be passed beside it."""
+    p, symbols, h_prev, parent = _step_inputs(dims)
+    base = _run_step(dims, p, symbols, h_prev, parent)
+    x_in = p["table"][symbols]
+    got = _run_step(dims, p, (symbols + 1) % p["table"].shape[0], h_prev, parent, x_in=x_in)
+    for name in base:
+        assert torch.equal(got[name], base[name]), name
+    assert torch.equal(got["x"].cpu(), x_in)
+
+
+@pytest.mark.parametrize("dims", STEP_DIMS)
+def test_step_kernel_without_optional_outputs(dims):
+    """x_out, ctx_out and weights_out NULL (as the decoding engine calls it): h_out and out unchanged."""
+    p, symbols, h_prev, parent = _step_inputs(dims)
+    base = _run_step(dims, p, symbols, h_prev, parent)
+    got = _run_step(dims, p, symbols, h_prev, parent, outputs=())
+    assert set(got) == {"h", "out"}
+    assert torch.equal(got["h"], base["h"]) and torch.equal(got["out"], base["out"])
 
 
 def test_step_kernel_rejects_null_pointers():
@@ -119,7 +178,8 @@ def _setup(cfg, backend, bsz, tx, ty, seed):
     return model, params, src, tgt
 
 
-@pytest.mark.parametrize("cfg,backend", [(TOY, "simt"), (MID, "simt"), (MID, "auto")])
+@pytest.mark.parametrize("cfg,backend", [(TOY, "simt"), (MID, "simt"), (MID, "auto"),
+                                         (dict(MID, out_act="relu"), "simt")])
 def test_fused_greedy_equals_the_stepwise_loop(cfg, backend):
     """Same symbols, masks, argmax and (to rounding) states / losses as the host loop over next_state; three
     decodes so that the CUDA-graph replay (from the second time a shape shows up) is compared too."""

@@ -22,6 +22,15 @@ def _weights(g, e, h, ws=0.3):
     return wg, bg, wc, bc
 
 
+def _reverse_sequence(x, lengths):
+    """tf.reverse_sequence(x, lengths, seq_axis=1) as one gather: O.reverse_sequence walks the batch row by row,
+    which autograd makes slow at a thousand rows."""
+    t = torch.arange(x.shape[1])[None, :]
+    n = lengths.long()[:, None]
+    idx = torch.where(t < n, n - 1 - t, t)
+    return x.gather(1, idx[:, :, None].expand(-1, -1, x.shape[2]))
+
+
 def _lengths(g, bsz, steps):
     lengths = torch.randint(1, steps + 1, (bsz,), generator=g)
     lengths[0] = steps
@@ -33,7 +42,10 @@ def _lengths(g, bsz, steps):
 SHAPES = [(1, 1, 8), (17, 50, 8), (256, 1, 8), (300, 50, 100), (1, 50, 100), (17, 1, 300), (256, 50, 300),
           (300, 1, 320), (17, 50, 320),
           # H where ceil(H/8) units per CTA would leave the last CTAs of a cluster without units
-          (17, 50, 9), (33, 20, 33), (5, 50, 49)]
+          (17, 50, 9), (33, 20, 33), (5, 50, 49),
+          # more clusters than are co-resident (15 on an H100): shared memory caps a cluster at 32 rows forward
+          # and 22 backward for H = 320, 68 and 42 for H = 100, so these run in several waves
+          (1024, 20, 320), (1100, 10, 100)]
 
 
 @pytest.mark.parametrize("shape", SHAPES)
@@ -60,8 +72,8 @@ def test_cluster_gru_vs_oracle(shape, variant):
         l64 = [t.double().requires_grad_(True) for t in tensors]
         h064 = l64[5] if h0 is not None else None
         if reverse:
-            out_rev, fin = O.dynamic_gru(O.reverse_sequence(l64[0], lengths), lengths, *l64[1:5], h0=h064)
-            ref_states = O.reverse_sequence(out_rev, lengths)
+            out_rev, fin = O.dynamic_gru(_reverse_sequence(l64[0], lengths), lengths, *l64[1:5], h0=h064)
+            ref_states = _reverse_sequence(out_rev, lengths)
         else:
             ref_states, fin = O.dynamic_gru(l64[0], lengths, *l64[1:5], h0=h064)
         assert max_abs(states, ref_states) < TOL
@@ -69,6 +81,54 @@ def test_cluster_gru_vs_oracle(shape, variant):
         ds, df = torch.randn(bsz, steps, h, generator=g), torch.randn(bsz, h, generator=g)
         ((states * ds.cuda()).sum() + (final * df.cuda()).sum()).backward()
         ((ref_states * ds.double()).sum() + (fin * df.double()).sum()).backward()
+        for got, want, name in zip(leaves, l64, ("x", "wg", "bg", "wc", "bc", "h0")):
+            assert rel_err(got.grad, want.grad) < GTOL, name
+    finally:
+        ops.set_gemm_backend("auto")
+
+
+@pytest.mark.parametrize("use_h0", [False, True])
+@pytest.mark.parametrize("reverse", [False, True])
+@pytest.mark.parametrize("shape", [(17, 12, 100), (9, 12, 300), (5, 8, 7), (6, 5, 330)])
+def test_gru_zero_lengths(shape, reverse, use_h0):
+    """Rows of length 0 among ragged ones, on the cluster kernels (H = 100, 300) and the per-step kernels (H = 7,
+    330), as tf.nn.dynamic_rnn treats them: zero outputs, the final state is h0 (zeros without one), dh0 is
+    dfinal and nothing flows into the inputs.  Those rows only carry values, so they compare exactly; the whole
+    layer compares with the oracle at the exact tolerances."""
+    from neuralmonkey_b200 import ops
+    bsz, steps, h = shape
+    e = 10
+    ops.set_gemm_backend("simt")
+    try:
+        g = torch.Generator().manual_seed(bsz * steps + h)
+        x = torch.randn(bsz, steps, e, generator=g)
+        wg, bg, wc, bc = _weights(g, e, h, ws=min(0.3, 1.0 / h ** 0.5))
+        lengths = torch.randint(1, steps + 1, (bsz,), generator=g)
+        lengths[0] = steps
+        zero = torch.arange(bsz) % 3 == 1
+        lengths[zero] = 0
+        h0 = torch.randn(bsz, h, generator=g) * 0.5 if use_h0 else None
+        tensors = (x, wg, bg, wc, bc) + ((h0,) if use_h0 else ())
+        leaves = [_leaf(t) for t in tensors]
+        states, final, _raw = ops.gru_layer(*leaves[:5], h0=leaves[5] if use_h0 else None,
+                                            lengths=lengths.to(torch.int32).cuda(), reverse=reverse)
+        l64 = [t.double().requires_grad_(True) for t in tensors]
+        h064 = l64[5] if use_h0 else None
+        if reverse:
+            out_rev, fin = O.dynamic_gru(_reverse_sequence(l64[0], lengths), lengths, *l64[1:5], h0=h064)
+            ref_states = _reverse_sequence(out_rev, lengths)
+        else:
+            ref_states, fin = O.dynamic_gru(l64[0], lengths, *l64[1:5], h0=h064)
+        assert torch.equal(states[zero.cuda()].cpu(), torch.zeros(int(zero.sum()), steps, h))
+        assert torch.equal(final[zero.cuda()].cpu(), h0[zero] if use_h0 else torch.zeros(int(zero.sum()), h))
+        assert max_abs(states, ref_states) < TOL
+        assert max_abs(final, fin) < TOL
+        ds, df = torch.randn(bsz, steps, h, generator=g), torch.randn(bsz, h, generator=g)
+        ((states * ds.cuda()).sum() + (final * df.cuda()).sum()).backward()
+        ((ref_states * ds.double()).sum() + (fin * df.double()).sum()).backward()
+        assert torch.equal(leaves[0].grad[zero.cuda()].cpu(), torch.zeros(int(zero.sum()), steps, e))
+        if use_h0:
+            assert torch.equal(leaves[5].grad[zero.cuda()].cpu(), df[zero])
         for got, want, name in zip(leaves, l64, ("x", "wg", "bg", "wc", "bc", "h0")):
             assert rel_err(got.grad, want.grad) < GTOL, name
     finally:

@@ -29,7 +29,12 @@ def test_embed_fwd_bwd():
     assert max_abs(td.grad, t64.grad) < 1e-5
 
 
-@pytest.mark.parametrize("dims", [(6, 14), (33, 600), (5, 1000)])
+# The kernels keep a row in registers, PER_LANE values per lane: classes D <= 256, 640, 1024 and 2048.  The widths
+# below are both sides of every class boundary and the ends; M = 5000 splits the parameter gradient into many
+# row chunks that meet by atomics.
+@pytest.mark.parametrize("dims", [(6, 14), (33, 600), (5, 1000),
+                                  (7, 1), (9, 32), (10, 33), (11, 256), (12, 257), (13, 640), (14, 641),
+                                  (15, 1024), (16, 1025), (17, 2048), (5000, 33), (5000, 1025)])
 def test_layer_norm_fwd_bwd(dims):
     from neuralmonkey_b200 import ops
     m, d = dims
@@ -46,6 +51,21 @@ def test_layer_norm_fwd_bwd(dims):
     assert rel_err(xd.grad, x64.grad) < 2e-5
     assert rel_err(gd.grad, g64.grad) < 2e-5
     assert rel_err(bd.grad, b64.grad) < 2e-5
+
+
+@pytest.mark.parametrize("d", [600, 1025])
+def test_layer_norm_two_pass_variance_at_an_offset(d):
+    """x = 100 + randn: the kernel subtracts the mean before it squares.  Replaying the kernel's fp32 summation
+    order (per-lane sums, then the warp butterfly) on the CPU puts y within ~4e-5 of fp64: the mean carries
+    the rounding of sums of values near 100, and y inherits it times rstd * gamma.  A one-pass
+    E[x^2] - E[x]^2 cancels two terms near 1e4 in fp32, is off by ~1e-3 in the unit variance and misses y by
+    ~7e-3."""
+    from neuralmonkey_b200 import ops
+    g = torch.Generator().manual_seed(d)
+    x = 100 + torch.randn(40, d, generator=g)
+    gamma, beta = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    y = ops.layer_norm(x.cuda(), gamma.cuda(), beta.cuda())
+    assert max_abs(y, O.layer_norm(x.double(), gamma.double(), beta.double())) < 1e-4
 
 
 @pytest.mark.parametrize("reverse", [False, True])
