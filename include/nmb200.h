@@ -614,6 +614,41 @@ int nm_sample_logits_step(const float* logits, int64_t ldl, float temperature, i
                           const uint8_t* finished_in, int64_t* symbols, uint8_t* finished_out, const int64_t* state,
                           int64_t loop_step, int64_t sample_index, int64_t rows, int64_t V, void* stream);
 
+/* ---- K18: sentence classification and regression (csrc/classify.cu) -------------------------------------------
+ * Time-major spans: sentence b, position t is row b*T + t of a [rows, D] matrix (D contiguous floats per row);
+ * mask [B,T] (0/1 floats) may be NULL (every position valid).  Reductions run in a fixed order: repeat calls give
+ * identical bits.
+ * nm_seq_max_pool_fwd: y[b,d] = max_{t<L} (x*m + 1e-15*(1-m)), i.e. reduce_max of encoders/pooling.py:49-57 (a
+ *   sentence whose valid values are all negative pools to 1e-15); relu != 0 gives max(y, 0), which is
+ *   reduce_max(relu(x)) of encoders/sequence_cnn_encoder.py:125-129.  1 <= L <= T.
+ * nm_seq_max_pool_bwd: TF's reduce_max gradient: dy split equally among ALL positions equal to the maximum, times
+ *   the mask; with relu, zero unless the maximum is positive (ReluGrad).  Writes every row r < rows of dx
+ *   (rows in [(B-1)*T + L, B*T]), zero at positions t >= L.
+ * nm_seq_mean_pool_fwd/bwd: y[b,d] = sum_t x*m / (sum_t m + 1e-8) (encoders/pooling.py:60-70).
+ * nm_attentive_pool_fwd: the self-attentive pooling of encoders/attentive.py:58-90 after its two dense layers:
+ *   energies [B,T,R], states [B,T,D]; weights [B,T,R] = softmax over all T positions, times the mask,
+ *   renormalised with +1e-8 (no renormalisation without a mask); out [B,R,D] = weights^T . states.
+ *   R <= 32 and T*R <= 16384, otherwise NM_E_UNSUPPORTED.
+ * nm_attentive_pool_bwd: from dout [B,R,D] (and dweights [B,T,R], may be NULL) and the forward's weights:
+ *   denergies [B,T,R] and dstates [B,T,D].
+ * nm_squared_error_fwd: loss[0] = mean over [B,dim] of (pred[b,i] - target[b])^2 (decoders/sequence_regressor.py:
+ *   78-87); nm_squared_error_bwd: dpred = dloss[0] * 2 (pred - target) / (B*dim), dloss a device scalar. */
+int nm_seq_max_pool_fwd(const float* x, const float* mask, float* y, int64_t B, int64_t L, int64_t T, int64_t D,
+                        int relu, void* stream);
+int nm_seq_max_pool_bwd(const float* x, const float* mask, const float* dy, float* dx, int64_t B, int64_t L,
+                        int64_t T, int64_t D, int64_t rows, int relu, void* stream);
+int nm_seq_mean_pool_fwd(const float* x, const float* mask, float* y, int64_t B, int64_t T, int64_t D, void* stream);
+int nm_seq_mean_pool_bwd(const float* mask, const float* dy, float* dx, int64_t B, int64_t T, int64_t D,
+                         void* stream);
+int nm_attentive_pool_fwd(const float* energies, const float* mask, const float* states, float* weights, float* out,
+                          int64_t B, int64_t T, int64_t R, int64_t D, void* stream);
+int nm_attentive_pool_bwd(const float* energies, const float* mask, const float* states, const float* weights,
+                          const float* dout, const float* dweights, float* denergies, float* dstates, int64_t B,
+                          int64_t T, int64_t R, int64_t D, void* stream);
+int nm_squared_error_fwd(const float* pred, const float* target, float* loss, int64_t B, int64_t dim, void* stream);
+int nm_squared_error_bwd(const float* pred, const float* target, const float* dloss, float* dpred, int64_t B,
+                         int64_t dim, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,8 @@ from typing import List, Tuple
 import torch
 
 from neuralmonkey_b200 import ops
+from neuralmonkey_b200.nn.projection import (activation_name, declare_multilayer_projection,
+                                             multilayer_projection)
 from neuralmonkey_b200.nn.utils import dropout
 from neuralmonkey_b200.params import zeros_initializer
 
@@ -102,37 +104,21 @@ class _MLP(OutputProjection):
         self.activation, self.dropout_keep_prob = activation, dropout_keep_prob
 
     def declare(self, decoder, in_size):
-        for i, width in enumerate(self.layer_sizes):
-            pre = "attention_decoder/deep_output_mlp/mlp_layer_{}/".format(i)
-            decoder.declare(pre + "kernel", [in_size, width])
-            decoder.declare(pre + "bias", [width], zeros_initializer())
-            in_size = width
+        declare_multilayer_projection(decoder, "attention_decoder/deep_output_mlp", in_size, self.layer_sizes)
 
     def __call__(self, decoder, prev_state, prev_output, ctx_tensors, train_mode):
         x = torch.cat([prev_state, prev_output] + list(ctx_tensors), -1)
-        for i in range(len(self.layer_sizes)):
-            pre = "attention_decoder/deep_output_mlp/mlp_layer_{}/".format(i)
-            # multilayer_projection (nn/projection.py:38-57): activation and dropout after EVERY layer
-            x = dropout(ops.linear(x, decoder.var(pre + "kernel"), decoder.var(pre + "bias"), act=self.activation),
-                        self.dropout_keep_prob, train_mode)
-        return x
-
-
-def _activation_name(activation_fn) -> str:
-    if callable(activation_fn):
-        activation_fn = getattr(activation_fn, "__name__", str(activation_fn))
-    if activation_fn not in ("tanh", "relu", "sigmoid"):
-        raise ValueError("Unsupported activation {}".format(activation_fn))
-    return activation_fn
+        return multilayer_projection(decoder, x, "attention_decoder/deep_output_mlp", self.layer_sizes,
+                                     self.activation, self.dropout_keep_prob, train_mode)
 
 
 def nematus_output(output_size: int, activation_fn: str = "tanh",
                    dropout_keep_prob: float = 1.0) -> Tuple[OutputProjection, int]:
     """activation(dense(state) + dense(embedding) + dense(contexts)) (output_projection.py:76-112)."""
-    return _Nematus(output_size, _activation_name(activation_fn), dropout_keep_prob), output_size
+    return _Nematus(output_size, activation_name(activation_fn), dropout_keep_prob), output_size
 
 
 def mlp_output(layer_sizes: List[int], activation: str = "tanh",
                dropout_keep_prob: float = 1.0) -> Tuple[OutputProjection, int]:
     """A multilayer perceptron over [state; embedding; contexts] (output_projection.py:163-188)."""
-    return _MLP(layer_sizes, _activation_name(activation), dropout_keep_prob), layer_sizes[-1]
+    return _MLP(layer_sizes, activation_name(activation), dropout_keep_prob), layer_sizes[-1]

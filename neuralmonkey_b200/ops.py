@@ -1429,3 +1429,196 @@ def pool2d(x: torch.Tensor, k: int, stride: int, padding: str, kind: str) -> tor
     if kind not in ("max", "avg"):
         raise ValueError("pooling kind must be 'max' or 'avg'")
     return _Pool2d.apply(x, int(k), int(stride), padding, kind == "max")
+
+
+# ---------------------------------------------------------------------------
+# K18 sentence classification and regression (csrc/classify.cu): pooling over time, self-attentive pooling,
+# the Kim-CNN convolution + max over time, the squared-error loss
+# ---------------------------------------------------------------------------
+def _mask_or_none(mask: Optional[torch.Tensor], b: int, t: int) -> Optional[torch.Tensor]:
+    if mask is None:
+        return None
+    if tuple(mask.shape) != (b, t):
+        raise ValueError("mask must be [{}, {}], got {}".format(b, t, tuple(mask.shape)))
+    return _f32(mask).contiguous()
+
+
+def _check_mask_sum(mask: Optional[torch.Tensor]) -> None:
+    """The reference's tf.assert_greater(reduce_sum(mask), 0.5) before its max pooling (encoders/pooling.py:53)."""
+    if mask is not None and float(mask.sum()) <= 0.5:
+        raise ValueError("max pooling over a batch without a single valid position (mask sum <= 0.5)")
+
+
+class _SeqMaxPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, mask):
+        b, t, d = x.shape
+        x = _f32(x).contiguous()
+        y = torch.empty(b, d, device=x.device, dtype=torch.float32)
+        call("nm_seq_max_pool_fwd", ptr(x), ptr(mask), ptr(y), b, t, t, d, 0, lib.stream())
+        ctx.save_for_backward(x, mask)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, mask = ctx.saved_tensors
+        b, t, d = x.shape
+        dx = torch.empty_like(x)
+        call("nm_seq_max_pool_bwd", ptr(x), ptr(mask), ptr(dy.contiguous()), ptr(dx), b, t, t, d, b * t, 0,
+             lib.stream())
+        return dx, None
+
+
+def seq_max_pool(x: torch.Tensor, mask: Optional[torch.Tensor]) -> torch.Tensor:
+    """reduce_max(x*m + 1e-15*(1-m), axis=1) of [B,T,D] x (SequenceMaxPooling); the gradient is split equally
+    among tied maxima, as TF's is."""
+    m = _mask_or_none(mask, x.shape[0], x.shape[1])
+    _check_mask_sum(m)
+    return _SeqMaxPool.apply(x, m)
+
+
+class _SeqMeanPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, mask):
+        b, t, d = x.shape
+        x = _f32(x).contiguous()
+        y = torch.empty(b, d, device=x.device, dtype=torch.float32)
+        call("nm_seq_mean_pool_fwd", ptr(x), ptr(mask), ptr(y), b, t, d, lib.stream())
+        ctx.save_for_backward(mask)
+        ctx.shape = (b, t, d)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (mask,) = ctx.saved_tensors
+        b, t, d = ctx.shape
+        dx = torch.empty(b, t, d, device=dy.device, dtype=torch.float32)
+        call("nm_seq_mean_pool_bwd", ptr(mask), ptr(dy.contiguous()), ptr(dx), b, t, d, lib.stream())
+        return dx, None
+
+
+def seq_mean_pool(x: torch.Tensor, mask: Optional[torch.Tensor]) -> torch.Tensor:
+    """sum_t(x*m) / (sum_t m + 1e-8) of [B,T,D] x (SequenceAveragePooling)."""
+    return _SeqMeanPool.apply(x, _mask_or_none(mask, x.shape[0], x.shape[1]))
+
+
+class _AttentivePool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, energies, mask, states):
+        b, t, r = energies.shape
+        d = states.shape[2]
+        energies, states = _f32(energies).contiguous(), _f32(states).contiguous()
+        weights = torch.empty(b, t, r, device=states.device, dtype=torch.float32)
+        out = torch.empty(b, r, d, device=states.device, dtype=torch.float32)
+        call("nm_attentive_pool_fwd", ptr(energies), ptr(mask), ptr(states), ptr(weights), ptr(out), b, t, r, d,
+             lib.stream())
+        ctx.save_for_backward(energies, mask, states, weights)
+        return weights, out
+
+    @staticmethod
+    def backward(ctx, dweights, dout):
+        energies, mask, states, weights = ctx.saved_tensors
+        b, t, r = energies.shape
+        d = states.shape[2]
+        if dout is None:
+            dout = torch.zeros(b, r, d, device=states.device, dtype=torch.float32)
+        de, ds = torch.empty_like(energies), torch.empty_like(states)
+        call("nm_attentive_pool_bwd", ptr(energies), ptr(mask), ptr(states), ptr(weights), ptr(dout.contiguous()),
+             ptr(None if dweights is None else dweights.contiguous()), ptr(de), ptr(ds), b, t, r, d, lib.stream())
+        return de, None, ds
+
+
+def attentive_pool(energies: torch.Tensor, mask: Optional[torch.Tensor],
+                   states: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The self-attentive pooling of AttentiveEncoder after its dense layers: energies [B,T,R], states [B,T,D] ->
+    (weights [B,T,R]: softmax over all T, times the mask, renormalised with +1e-8; weights^T . states [B,R,D])."""
+    if energies.dim() != 3 or states.dim() != 3 or energies.shape[:2] != states.shape[:2]:
+        raise ValueError("energies [B,T,R] and states [B,T,D] must agree on B and T, got {} and {}".format(
+            tuple(energies.shape), tuple(states.shape)))
+    return _AttentivePool.apply(energies, _mask_or_none(mask, energies.shape[0], energies.shape[1]), states)
+
+
+class _Conv1dMaxPool(torch.autograd.Function):
+    """y[m] = sum_j x_flat[m+j] . w[j] + bias over the M = B*T-w+1 rows of the flattened batch: one nm_gemm per
+    filter tap over a row-shifted view of x (K = E each), accumulated in place (beta = 1).  The windows that cross a
+    sentence boundary are computed and never read.  The ReLU is folded into the max over time (max(relu(y)) =
+    relu(max(y)), and the ReLU gradient at the tied positions)."""
+
+    @staticmethod
+    def forward(ctx, x, w, bias):
+        b, t, e = x.shape
+        width, _, f = w.shape
+        x2 = _f32(x).contiguous().view(b * t, e)
+        m = b * t - width + 1
+        y = torch.empty(m, f, device=x.device, dtype=torch.float32)
+        for j in range(width):
+            gemm(x2[j:j + m], w[j], y, bias=bias if j == 0 else None, beta=0.0 if j == 0 else 1.0)
+        out = torch.empty(b, f, device=x.device, dtype=torch.float32)
+        call("nm_seq_max_pool_fwd", ptr(y), None, ptr(out), b, t - width + 1, t, f, 1, lib.stream())
+        ctx.save_for_backward(x2, w, y)
+        ctx.shape = (b, t, e, width, f)
+        ctx.sinks = (_sink(w), _sink(bias))
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x2, w, y = ctx.saved_tensors
+        b, t, e, width, f = ctx.shape
+        m = y.shape[0]
+        dy = torch.empty_like(y)
+        call("nm_seq_max_pool_bwd", ptr(y), None, ptr(dout.contiguous()), ptr(dy), b, t - width + 1, t, f, m, 1,
+             lib.stream())
+        w_sink, b_sink = ctx.sinks
+        dw = None if w_sink is not None else torch.empty_like(w)
+        for j in range(width):
+            if w_sink is not None:
+                gemm(x2[j:j + m], dy, w_sink[j], trans_a=True, beta=1.0)
+            else:
+                gemm(x2[j:j + m], dy, dw[j], trans_a=True)
+        db = _bias_grad(dy, b_sink)
+        dx = torch.zeros(b * t, e, device=y.device, dtype=torch.float32)
+        for j in range(width):
+            gemm(dy, w[j], dx[j:j + m], trans_b=True, beta=1.0)
+        return dx.view(b, t, e), dw, db
+
+
+def conv1d_max_pool(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """reduce_max(relu(conv1d(x, w, VALID) + bias), axis=1) of the Kim-CNN sentence encoder: x [B,T,E],
+    w [width,E,F], bias [F] -> [B,F].  A batch shorter than the filter is refused (TF would reduce over an empty
+    axis)."""
+    b, t, e = x.shape
+    if w.dim() != 3 or w.shape[1] != e or bias.shape != (w.shape[2],):
+        raise ValueError("conv1d_max_pool: filter {} and bias {} do not fit inputs of width {}".format(
+            tuple(w.shape), tuple(bias.shape), e))
+    if t < w.shape[0]:
+        raise ValueError("the batch is {} positions long, shorter than the filter width {}: the max over time "
+                         "would run over no window".format(t, w.shape[0]))
+    return _Conv1dMaxPool.apply(x, w, bias)
+
+
+class _SquaredError(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pred, target):
+        b, dim = pred.shape
+        pred, target = _f32(pred).contiguous(), _f32(target).contiguous()
+        loss = torch.empty((), device=pred.device, dtype=torch.float32)
+        call("nm_squared_error_fwd", ptr(pred), ptr(target), ptr(loss), b, dim, lib.stream())
+        ctx.save_for_backward(pred, target)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        pred, target = ctx.saved_tensors
+        b, dim = pred.shape
+        dpred = torch.empty_like(pred)
+        call("nm_squared_error_bwd", ptr(pred), ptr(target), ptr(dloss.contiguous()), ptr(dpred), b, dim,
+             lib.stream())
+        return dpred, None
+
+
+def squared_error(pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+    """mean((pred [B,dim] - target[:, None])^2), the SequenceRegressor cost."""
+    if pred.dim() != 2 or target.shape != (pred.shape[0],):
+        raise ValueError("squared_error: predictions [B, dim] and targets [B], got {} and {}".format(
+            tuple(pred.shape), tuple(target.shape)))
+    return _SquaredError.apply(pred, target)
