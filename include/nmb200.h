@@ -649,6 +649,33 @@ int nm_squared_error_fwd(const float* pred, const float* target, float* loss, in
 int nm_squared_error_bwd(const float* pred, const float* target, const float* dloss, float* dpred, int64_t B,
                          int64_t dim, void* stream);
 
+/* ---- K19: one layer of the convolutional seq2seq encoder (encoders/facebook_conv.py, csrc/glu_conv.cu) ----------
+ * x [B,T,F], w [k,F,2F], bias [2F], fp32, row-major; M = B*T.
+ *   z = conv1d(x, w) + bias       TF's SAME padding at stride 1: (k-1)/2 zeros before each sequence, the rest after;
+ *                                 positions inside [0,T) always take part, padded batch positions included
+ *   y = z[..., :F] * sigmoid(z[..., F:]) + x
+ * Any B, T (T < k and T = 1 included), F and k.  backend: NM_GEMM_SIMT = exact fp32 on the CUDA cores,
+ * NM_GEMM_AUTO / NM_GEMM_TC = wgmma with TF32 operands.  Implicit GEMMs: no patch matrix.
+ * nm_glu_conv1d_fwd: y [B,T,F]; z [B,T,2F] is written only when non-NULL (training keeps it for the backward).
+ * nm_glu_conv1d_dz: dz [M,2F] = the gradient of z from dy [M,F] and the saved z.
+ * nm_glu_conv1d_dgrad: dx [B,T,F] = conv1d of dz with w's taps reversed and channel axes swapped, + dy (the
+ * residual); dx must not alias dz or dy.
+ * nm_glu_conv1d_wgrad: dw [k,F,2F] += sum over positions of patch(x)^T dz, db [2F] += sum dz.  The position sum is
+ * split over CTAs into `workspace` (>= (k*F+1)*2F floats; more lets it split further) and the partials are added
+ * in a fixed order: two calls give identical bits.  db is that product's row of ones, so on the wgmma engine it sums
+ * dz rounded to TF32 like every other operand (2^-11 relative per term); NM_GEMM_SIMT sums it in fp32.
+ * nm_glu_conv1d_wgrad_workspace: the workspace (floats) at which nm_glu_conv1d_wgrad splits as far as it wants to
+ * for that shape and backend, or -1 for invalid sizes. */
+int nm_glu_conv1d_fwd(const float* x, const float* w, const float* bias, float* y, float* z, int64_t B, int64_t T,
+                      int64_t F, int64_t k, int backend, void* stream);
+int nm_glu_conv1d_dz(const float* dy, const float* z, float* dz, int64_t M, int64_t F, void* stream);
+int nm_glu_conv1d_dgrad(const float* dz, const float* w, const float* dy, float* dx, int64_t B, int64_t T, int64_t F,
+                        int64_t k, int backend, void* stream);
+int64_t nm_glu_conv1d_wgrad_workspace(int64_t B, int64_t T, int64_t F, int64_t k, int backend);
+int nm_glu_conv1d_wgrad(const float* x, const float* dz, float* dw, float* db, float* workspace,
+                        int64_t workspace_floats, int64_t B, int64_t T, int64_t F, int64_t k, int backend,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

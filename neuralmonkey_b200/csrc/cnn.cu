@@ -69,14 +69,6 @@ constexpr int CT_A_BYTES = CT_BM * 128, CT_B_BYTES = CT_BN * 128;
 constexpr int CT_STAGE = CT_A_BYTES + CT_B_BYTES;
 constexpr int CT_SMEM = 2 * CT_STAGE + 1024;   // + slack for the 1 KB alignment of the swizzled tiles
 
-__device__ __forceinline__ void sw128_store4(uint8_t* tile, int row, int chunk, float4 v) {
-  uint4 u = make_uint4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
-  *reinterpret_cast<uint4*>(tile + row * 128 + ((chunk ^ (row & 7)) << 4)) = u;
-}
-__device__ __forceinline__ void sw128_store1(uint8_t* tile, int row, int word, float v) {
-  *reinterpret_cast<uint32_t*>(tile + row * 128 + (((word >> 2) ^ (row & 7)) << 4) + ((word & 3) << 2)) = to_tf32(v);
-}
-
 // Each warpgroup multiplies its 64 rows of the stage's A tile by the B tile (4 instructions of k = 8).
 __device__ __forceinline__ void ct_mma(float (&acc)[32], uint32_t stage_addr, int wg) {
   const uint32_t a = stage_addr + wg * 64 * 128, b = stage_addr + CT_A_BYTES;

@@ -97,4 +97,14 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t addr) {
          ((uint64_t)1 << 62);
 }
 
+// Stores into a K-major tile in the 128-byte swizzle (rows of 32 tf32 words), rounding to TF32 (cvt.rna): four
+// words of 16-byte chunk `chunk`, or the single word `word`.
+__device__ __forceinline__ void sw128_store4(uint8_t* tile, int row, int chunk, float4 v) {
+  uint4 u = make_uint4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
+  *reinterpret_cast<uint4*>(tile + row * 128 + ((chunk ^ (row & 7)) << 4)) = u;
+}
+__device__ __forceinline__ void sw128_store1(uint8_t* tile, int row, int word, float v) {
+  *reinterpret_cast<uint32_t*>(tile + row * 128 + (((word >> 2) ^ (row & 7)) << 4) + ((word & 3) << 2)) = to_tf32(v);
+}
+
 }  // namespace nm

@@ -1346,6 +1346,63 @@ def conv2d(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], padding:
     return _Conv2d.apply(x, w, b, padding, act)
 
 
+def glu_conv_wgrad_workspace(bsz, t, f, k, backend) -> int:
+    want = int(lib.load().nm_glu_conv1d_wgrad_workspace(bsz, t, f, k, backend))
+    if want < 0:
+        raise ValueError("conv1d_glu_residual: bad sizes {}".format((bsz, t, f, k)))
+    return max((k * f + 1) * 2 * f, min(_WGRAD_WS_FLOATS, want))
+
+
+class _Conv1dGluResidual(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b):
+        bsz, t, f = x.shape
+        k = w.shape[0]
+        if w.shape[1:] != (f, 2 * f) or tuple(b.shape) != (2 * f,):
+            raise ValueError("conv1d_glu_residual: filter {} / bias {} do not fit input {}".format(
+                tuple(w.shape), tuple(b.shape), tuple(x.shape)))
+        x = _f32(x).contiguous()
+        w = _f32(w).contiguous()
+        b = _f32(b).contiguous()
+        y = torch.empty_like(x)
+        training = any(ctx.needs_input_grad)
+        z = torch.empty(bsz, t, 2 * f, device=x.device, dtype=torch.float32) if training else None
+        backend = _conv_backend()
+        call("nm_glu_conv1d_fwd", ptr(x), ptr(w), ptr(b), ptr(y), ptr(z), bsz, t, f, k, backend, lib.stream())
+        ctx.save_for_backward(x, w, z)
+        ctx.geom = (bsz, t, f, k, backend)
+        ctx.sinks = (_sink(w), _sink(b))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, z = ctx.saved_tensors
+        bsz, t, f, k, backend = ctx.geom
+        dy = _f32(dy).contiguous()
+        dz = torch.empty_like(z)
+        call("nm_glu_conv1d_dz", ptr(dy), ptr(z), ptr(dz), bsz * t, f, lib.stream())
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            call("nm_glu_conv1d_dgrad", ptr(dz), ptr(w), ptr(dy), ptr(dx), bsz, t, f, k, backend, lib.stream())
+        w_sink, b_sink = ctx.sinks
+        if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
+            return dx, None, None
+        dw = w_sink if w_sink is not None else torch.zeros_like(w)
+        db = b_sink if b_sink is not None else torch.zeros(2 * f, device=x.device, dtype=torch.float32)
+        ws = torch.empty(glu_conv_wgrad_workspace(bsz, t, f, k, backend), device=x.device, dtype=torch.float32)
+        call("nm_glu_conv1d_wgrad", ptr(x), ptr(dz), ptr(dw), ptr(db), ptr(ws), ws.numel(), bsz, t, f, k, backend,
+             lib.stream())
+        return dx, None if w_sink is not None else dw, None if b_sink is not None else db
+
+
+def conv1d_glu_residual(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """One ConvS2S encoder layer: z = tf.nn.conv1d(x, w, 1, 'SAME') + b, y = z[..., :F] * sigmoid(z[..., F:]) + x.
+    x [B,T,F], w [k,F,2F], b [2F].  The exact fp32 kernels under the 'simt' GEMM backend, wgmma with TF32 operands
+    otherwise."""
+    return _Conv1dGluResidual.apply(x, w, b)
+
+
 BN_WS_DOUBLES_PER_CHANNEL = 130     # NM_BN_WS_DOUBLES_PER_CHANNEL
 
 
