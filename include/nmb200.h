@@ -81,6 +81,9 @@ int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K,
 /* 1 if nm_gemm(AUTO) would take the wgmma path for this problem. */
 int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K,
                     int64_t lda, int64_t ldb, int64_t ldc);
+/* The wgmma plan nm_gemm would use for a dense product: tile width, number of split-K slices and
+ * k-blocks (32 fp32 elements) per slice.  sms <= 0: this device's SM count. */
+int nm_gemm_tc_plan(int64_t M, int64_t N, int64_t K, int act, int sms, int* bn, int* splits, int* kb_per_split);
 
 /* dst[c * ld_dst + r] = tf32(src[r * ld_src + c]) for a [rows, cols] source (a strided column slice is fine):
  * the transpose of src rounded to TF32 with cvt.rna (low 13 bits zero), i.e. the K-major copy of an operand

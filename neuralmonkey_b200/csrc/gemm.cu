@@ -30,6 +30,19 @@ int nm_gemm_uses_tc(int transA, int transB, int64_t M, int64_t N, int64_t K, int
   return tc_gemm_supported(M, N, K, lda, ldb, nullptr, nullptr) ? 1 : 0;
 }
 
+int nm_gemm_tc_plan(int64_t M, int64_t N, int64_t K, int act, int sms, int* bn, int* splits, int* kb_per_split) {
+  NM_REQUIRE(bn && splits && kb_per_split, NM_E_INVALID, "nm_gemm_tc_plan: null output");
+  NM_REQUIRE(M >= 1 && N >= 1 && K >= 1 && M <= 0x7fffffffLL && N <= 0x7fffffffLL && K <= 0x7fffffffLL,
+             NM_E_INVALID, "nm_gemm_tc_plan: bad shape %lld x %lld x %lld", (long long)M, (long long)N,
+             (long long)K);
+  NM_REQUIRE(act >= NM_ACT_NONE && act <= NM_ACT_SIGMOID, NM_E_INVALID, "nm_gemm_tc_plan: unknown act %d", act);
+  const TcPlan p = tc_dense_plan(M, N, K, act, sms > 0 ? sms : sm_count());
+  *bn = p.bn;
+  *splits = p.splits;
+  *kb_per_split = p.kb_per;
+  return NM_OK;
+}
+
 int nm_gemm(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda,
             const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, int act,
             float beta, int backend, void* stream) {

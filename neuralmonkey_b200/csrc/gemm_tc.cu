@@ -861,7 +861,7 @@ int tc_gemm_batched_launch(int transA, int transB, int64_t M, int64_t N, int64_t
   return launch_bn<false, true, TC_EPI_DENSE, 4>(bn, ma, mb, oa, ob, M, N, K, epi, 1, 0, TcExt{}, bt, s, name);
 }
 
-static int pick_bn(int64_t M, int64_t N, int64_t K) {
+static int pick_bn(int64_t M, int64_t N, int64_t K, int sms) {
   if (N <= 64) return 64;
   if (N <= 128) return 128;
   // skinny output, very long reduction (dX of the vocabulary projection: 12800 x 300 x 32000):
@@ -869,9 +869,41 @@ static int pick_bn(int64_t M, int64_t N, int64_t K) {
   if (K >= 8192 && N > 256 && N <= 320) return 160;
   const int64_t pad128 = ceil_div(N, 128) * 128, pad256 = ceil_div(N, 256) * 256;
   const int64_t tiles256 = ceil_div(M, TC_BM) * ceil_div(N, 256);
-  if (pad256 == pad128 && tiles256 >= sm_count()) return 256;
-  if (pad256 * 10 <= pad128 * 11 && tiles256 >= 2 * (int64_t)sm_count()) return 256;
+  if (pad256 == pad128 && tiles256 >= sms) return 256;
+  if (pad256 * 10 <= pad128 * 11 && tiles256 >= 2 * (int64_t)sms) return 256;
   return 128;
+}
+
+TcPlan tc_dense_plan(int64_t M, int64_t N, int64_t K, int act, int sms) {
+  const int bn = pick_bn(M, N, K, sms);
+  // split-K when the output alone cannot occupy the chip (and nothing forbids partial sums)
+  int splits = 1;
+  int kb_per = (int)ceil_div(K, TC_BK);
+  const int64_t tiles = ceil_div(M, TC_BM) * ceil_div(N, bn);
+  const int64_t num_kb = ceil_div(K, TC_BK);
+  if (act == NM_ACT_NONE && tiles * 2 <= sms && num_kb >= 16) {
+    int64_t want = ceil_div(sms, tiles);
+    if (want > num_kb / 8) want = num_kb / 8;
+    if (want > 1) {
+      kb_per = (int)ceil_div(num_kb, want);
+      splits = (int)ceil_div(num_kb, kb_per);  // every split owns >= 1 k-block
+    }
+  } else if (act == NM_ACT_NONE && num_kb >= 256 && tiles < 4 * (int64_t)sms) {
+    // a few waves of very long tiles: the last, partly filled wave costs a whole tile time.
+    // Cut K so that the work items fill the waves (static round-robin: ceil(items/SMs) rounds).
+    int best = 1;
+    double best_cost = (double)ceil_div(tiles, sms);
+    for (int sp = 2; sp <= 8; ++sp) {
+      if (num_kb / sp < 64) break;
+      const double cost = (double)ceil_div(tiles * sp, sms) / sp;
+      if (cost < best_cost * 0.93) { best_cost = cost; best = sp; }
+    }
+    if (best > 1) {
+      kb_per = (int)ceil_div(num_kb, best);
+      splits = (int)ceil_div(num_kb, kb_per);
+    }
+  }
+  return TcPlan{bn, splits, kb_per};
 }
 
 int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A,
@@ -881,36 +913,9 @@ int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, cons
   // op(B) is [K,N]: transB=0 -> B stored [K,N], N contiguous (MN-major);
   //                 transB=1 -> B stored [N,K], K contiguous (K-major).
   const bool a_mn = transA != 0, b_mn = transB == 0;
-  const int bn = (epi.mode == TC_EPI_DENSE) ? pick_bn(M, N, K) : TC_XENT_BN;
-  // split-K when the output alone cannot occupy the chip (and nothing forbids partial sums)
-  int splits = 1;
-  int kb_per = (int)ceil_div(K, TC_BK);
-  if (epi.mode == TC_EPI_DENSE) {
-    const int64_t tiles = ceil_div(M, TC_BM) * ceil_div(N, bn);
-    const int64_t num_kb = ceil_div(K, TC_BK);
-    if (epi.act == NM_ACT_NONE && tiles * 2 <= sm_count() && num_kb >= 16) {
-      int64_t want = ceil_div(sm_count(), tiles);
-      if (want > num_kb / 8) want = num_kb / 8;
-      if (want > 1) {
-        kb_per = (int)ceil_div(num_kb, want);
-        splits = (int)ceil_div(num_kb, kb_per);  // every split owns >= 1 k-block
-      }
-    } else if (epi.act == NM_ACT_NONE && num_kb >= 256 && tiles < 4 * (int64_t)sm_count()) {
-      // a few waves of very long tiles: the last, partly filled wave costs a whole tile time.
-      // Cut K so that the work items fill the waves (static round-robin: ceil(items/SMs) rounds).
-      int best = 1;
-      double best_cost = (double)ceil_div(tiles, sm_count());
-      for (int sp = 2; sp <= 8; ++sp) {
-        if (num_kb / sp < 64) break;
-        const double cost = (double)ceil_div(tiles * sp, sm_count()) / sp;
-        if (cost < best_cost * 0.93) { best_cost = cost; best = sp; }
-      }
-      if (best > 1) {
-        kb_per = (int)ceil_div(num_kb, best);
-        splits = (int)ceil_div(num_kb, kb_per);
-      }
-    }
-  }
+  const TcPlan plan = epi.mode == TC_EPI_DENSE ? tc_dense_plan(M, N, K, epi.act, sm_count())
+                                               : TcPlan{TC_XENT_BN, 1, (int)ceil_div(K, TC_BK)};
+  const int bn = plan.bn, splits = plan.splits, kb_per = plan.kb_per;
   CUtensorMap ma, mb;
   TcOperand oa, ob;
   int rc = a_mn ? make_operand(&ma, &oa, true, A, K, M, lda, TC_BM, 4) : make_operand(&ma, &oa, false, A, M, K, lda, TC_BM, 4);

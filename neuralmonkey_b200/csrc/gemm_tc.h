@@ -88,6 +88,13 @@ int xent16_launch(bool bwd, const void* X16, int64_t ldx, const void* WT16, int6
 // True when the operands can be addressed by TMA (16-byte aligned rows and bases).
 bool tc_gemm_supported(int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, const void* A, const void* B);
 
+// How tc_gemm_launch runs a dense product on `sms` SMs: bn-column tiles, and the reduction cut into `splits`
+// slices of kb_per k-blocks (32 fp32 elements) whose partial tiles are added into C (splits = 1: no cut).
+struct TcPlan {
+  int bn, splits, kb_per;
+};
+TcPlan tc_dense_plan(int64_t M, int64_t N, int64_t K, int act, int sms);
+
 // op(A)[M,K] . op(B)[K,N] with the given epilogue.  Same operand conventions as nm_gemm.
 int tc_gemm_launch(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A,
                    int64_t lda, const float* B, int64_t ldb, const TcEpilogue& epi, cudaStream_t s);

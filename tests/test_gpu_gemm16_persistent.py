@@ -47,7 +47,7 @@ def _gemm_f16(m, n, k, transposed, beta, row_scale=True, seed=1, a_scale=0.5):
     return _rel(c, want)
 
 
-@pytest.mark.parametrize("m,n,k", [
+F16_SHAPES = [
     (12800, 300, 32000),     # dX of the bench step: 100 tiles of 500 k-blocks, every tile cut between CTAs
     (2048, 300, 32000),
     (1000, 300, 640),        # 80 k-blocks in all: one per CTA, every tile summed from ten pieces
@@ -56,7 +56,10 @@ def _gemm_f16(m, n, k, transposed, beta, row_scale=True, seed=1, a_scale=0.5):
     (333, 321, 517),         # one column into a second column tile
     (40, 77, 1030),          # fewer rows than one warpgroup's 64
     (200, 600, 90),
-])
+]
+
+
+@pytest.mark.parametrize("m,n,k", F16_SHAPES)
 @pytest.mark.parametrize("transposed,beta", [(0, 0.0), (0, 1.0), (1, 0.0), (1, 1.0)])
 def test_gemm_f16_persistent(m, n, k, transposed, beta):
     # fp32 accumulation: over 32000 products about 2e-5 here (4e-5 on the one-CTA-per-tile kernel this replaced)
@@ -84,7 +87,7 @@ def _gemm_f16_tn(m, n, k, beta, seed=3, c_offset=0, b_scale=0.5):
     return _rel(c, want)
 
 
-@pytest.mark.parametrize("m,n,k,c_offset", [
+F16_TN_SHAPES = [
     (301, 32000, 12800, 3),    # [dW; db] of the bench step into the gradient buffer: C^T = B^T A, 250 x 200 k-blocks
     (301, 32000, 2048, 90000),
     (301, 4100, 640, 1),       # tiles cut between CTAs
@@ -93,7 +96,10 @@ def _gemm_f16_tn(m, n, k, beta, seed=3, c_offset=0, b_scale=0.5):
     (321, 1000, 517, 0),
     (40, 260, 1030, 0),        # fewer than 64 of the smaller dimension
     (1000, 333, 300, 1),       # M > N: M down the rows, no transposed store
-])
+]
+
+
+@pytest.mark.parametrize("m,n,k,c_offset", F16_TN_SHAPES)
 @pytest.mark.parametrize("beta", [0.0, 1.0])
 def test_gemm_f16_tn_persistent(m, n, k, c_offset, beta):
     assert _gemm_f16_tn(m, n, k, beta, c_offset=c_offset) < 5e-5
