@@ -7,15 +7,16 @@
 // 32 lanes keeps, in REGISTERS, the three weight vectors of those 4 units restricted to
 // ONE of 32 reduction slices of SL = ceil(H/32) elements (3 * 4 * SL floats per thread, 120
 // at H = 300).  The inner product streams only the state vector from shared memory in 16-,
-// 8- and 4-byte pieces of exactly SL elements and is FMA-issue bound.  The 32 partial sums
+// 8- or 4-byte pieces of exactly SL elements and is FMA-issue bound.  The 32 partial sums
 // of a (row, unit) pair are combined with a reduce-scatter over shuffles.
 //
 // The two matmuls of a TF GRUCell step are dependent (the candidate needs r*h for ALL
-// units).  The lanes that end up holding a reduced sum apply the gate math themselves and
-// write the result - r*h or h' forward, dz_c / dz_u / dz_r backward - straight into the
-// vector buffer of every CTA of the cluster with st.async, whose bytes are counted on a
-// transaction mbarrier of the receiving CTA.  A CTA starts a phase as soon as its barrier has
-// counted the whole Bc x H vector: no cluster-wide barrier and no L2 round trip in the loop.
+// units).  The lanes that end up holding a reduced sum apply the gate math themselves; the
+// four results of a warp's units in one row - r*h or h' forward, dz_c / dz_u / dz_r backward -
+// are gathered into one lane per destination and written straight into the vector buffer of
+// every CTA of the cluster as ONE 16-byte st.async, whose bytes are counted on a transaction
+// mbarrier of the receiving CTA.  A CTA starts a phase as soon as its barrier has counted the
+// whole Bc x H vector: no cluster-wide barrier and no L2 round trip in the loop.
 // Write-after-read hazards are ordered by the dataflow itself: a peer can only send the next
 // value of a buffer after it has received this CTA's contribution to the phase that follows
 // the last read of that buffer; the buffers for which that is not enough (forward h,
@@ -40,9 +41,9 @@ constexpr int GC_BAR_BYTES = 64;  // transaction barriers at the start of dynami
 constexpr int GC_XS = 4;        // forward prefetch per (row, unit): xproj r, u, c and the dropout mask
 constexpr int GC_PF = 8;        // backward prefetch per (row, unit): r, u, c, h, dstates, drop mask, draw
 
-// Geometry: SLP = slice pitch in the smem vector buffer, an odd number of 16-byte chunks so
-// the 32 lanes of a 16-byte load fall into 4 conflict-free quarter-warp wavefronts;
-// ROW = 32*SLP floats per batch row.  Only the first SL floats of a slice are ever read.
+// Row pitch of the smem vector buffers in floats: 32 * 4 * (ceil(SL/4) | 1) >= the 32 * SL floats a
+// row of the layout below uses.  The shared-memory plan, and with it the rows a cluster may take,
+// is sized from it.
 __host__ __device__ constexpr int gc_row(int SL) { return GC_SLICES * 4 * (((SL + 3) / 4) | 1); }
 // floats of dynamic shared memory per batch row, after the barrier block
 __host__ __device__ constexpr int gc_fwd_row_floats(int SL) {
@@ -52,12 +53,23 @@ __host__ __device__ constexpr int gc_bwd_row_floats(int SL) {
   return 4 * gc_row(SL) + GC_MAX_UNITS * (1 + 2 * GC_PF) + 1;
 }
 
+// Layout of an exchanged vector in a row: 8 rank regions of UP = 4*SL floats (UP >= ceil(H/8), a
+// multiple of 4), local unit i of CTA r at r*UP + i, so the 4 units of warp w are the 16-byte aligned
+// quad at r*UP + 4w.  Lane l's reduction slice is the SL consecutive floats at l*SL; positions past a
+// CTA's units hold 0 in the buffers and in the weights.
+// Slices are read in pieces of V floats, as wide as their alignment allows.  At SL = 8 the 16-byte
+// pieces of lanes 4 apart fall on the same banks, so lanes with bit 2 set read their two pieces in
+// the other order (the weights are loaded in the same order); every other SL is conflict-free as is.
 template <int SL>
 struct GcGeom {
-  static constexpr int SLP = 4 * (((SL + 3) / 4) | 1);
-  static constexpr int ROW = GC_SLICES * SLP;
-  // offset of hidden unit j inside a row of the sliced layout
-  static __device__ __forceinline__ int pos(int j) { return (j / SL) * SLP + (j % SL); }
+  static constexpr int UP = 4 * SL;
+  static constexpr int ROW = gc_row(SL);
+  static constexpr int V = SL % 4 == 0 ? 4 : SL % 2 == 0 ? 2 : 1;
+  // row offset of element e of lane `lane`'s slice
+  static __device__ __forceinline__ int slice_pos(int lane, int e) {
+    const int swz = SL == 8 ? ((lane >> 2) & 1) * 4 : 0;
+    return lane * SL + (e ^ swz);
+  }
 };
 
 __device__ __forceinline__ void cluster_barrier() {
@@ -106,6 +118,45 @@ __device__ __forceinline__ void gc_send(uint32_t addr, uint32_t bar, uint32_t ds
                "r"(__float_as_uint(v)), "r"(rb)
                : "memory");
 }
+// The same for the 16-byte aligned quad v at `addr`: one message of 16 bytes.
+__device__ __forceinline__ void gc_send4(uint32_t addr, uint32_t bar, uint32_t dst, const float (&v)[4]) {
+  uint32_t ra, rb;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(addr), "r"(dst));
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(bar), "r"(dst));
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::
+                   "r"(ra), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
+               "r"(__float_as_uint(v[3])), "r"(rb)
+               : "memory");
+}
+// q[u] = x of lane (L & KEEP) | (STRIDE * u), u = 0..3, for the calling lane L: the quad a sending lane
+// passes to gc_send4.  KEEP is the segment mask of shfl.sync, which may be any set of lane bits; with
+// the source lane an immediate, the shuffles hold no index registers.
+template <int KEEP, int SRC>
+__device__ __forceinline__ float gc_shfl_keep(float x) {
+  uint32_t o;
+  asm volatile("shfl.sync.idx.b32 %0, %1, %2, %3, 0xffffffff;"
+               : "=r"(o)
+               : "r"(__float_as_uint(x)), "n"(SRC), "n"((KEEP << 8) | 0x1f));
+  return __uint_as_float(o);
+}
+template <int KEEP, int STRIDE>
+__device__ __forceinline__ void gc_gather4(float (&q)[4], float x) {
+  static_assert((KEEP & (3 * STRIDE)) == 0, "the unit bits of the source lane come from STRIDE * u");
+  q[0] = gc_shfl_keep<KEEP, 0>(x);
+  q[1] = gc_shfl_keep<KEEP, STRIDE>(x);
+  q[2] = gc_shfl_keep<KEEP, 2 * STRIDE>(x);
+  q[3] = gc_shfl_keep<KEEP, 3 * STRIDE>(x);
+}
+// Bytes of one exchanged Bc x H vector as the live warps of the 8 CTAs send it: per row, one quad
+// per live warp, ceil(UW_r / 4) of them in CTA r.  Recomputed from the kernel parameters where it is
+// used, so that it holds no register across the step loop (the SL = 10 instance is at the
+// 168-register cap).
+__device__ __forceinline__ uint32_t gc_quad_bytes(int H, int Bc) {
+  int quads = 0;
+#pragma unroll
+  for (int r = 0; r < GC_CLUSTER; ++r) quads += ((r + 1) * H / GC_CLUSTER - r * H / GC_CLUSTER + 3) / 4;
+  return (uint32_t)(Bc * 16 * quads);
+}
 
 __device__ __forceinline__ void cp_async4(float* smem_dst, const float* gmem_src) {
   const uint32_t d = gc_smem_u32(smem_dst);
@@ -114,17 +165,20 @@ __device__ __forceinline__ void cp_async4(float* smem_dst, const float* gmem_src
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// Sum N values across the 32 lanes with N-1+log2(32/N)... shuffles instead of 5N: each
-// butterfly level halves the number of live values (lanes whose bit `o` is set keep the
-// upper half and send the lower, and vice versa).  On return v[0] of lane L is the full
-// sum of the value with index (L >> (5 - log2 N)) & (N-1); lanes differing only in the
-// low bits hold copies.
+// Sum N values (index = gate*8 + row*4 + unit) across the 32 lanes with N-1+log2(32/N)...
+// shuffles instead of 5N: each butterfly level halves the number of live values.  On return v[0]
+// of lane L is the full sum of the value with index (L >> (5 - log2 N)) & (N-1); lanes differing
+// only in the low bits hold copies.  At the row level, lanes whose bit `O` is set keep the upper
+// half and send the lower, and vice versa.  At the gate and unit levels every lane keeps the lower
+// half: that sums matching values because the caller permutes the slots there - slot g*8 + r*4 + u
+// holds gate g ^ g_L and unit u ^ u_L, the ones lane L ends up with - where the weights are loaded,
+// so those levels cost no select.
 // One butterfly level per instantiation, O = shuffle distance (a loop over the levels is not
 // always unrolled, and a rolled loop indexes v at run time, which puts v in local memory).
 template <int N, int O>
 __device__ __forceinline__ void gc_reduce_level(float (&v)[N], int lane) {
   constexpr int n = N * O / 16;  // values still live at this level
-  if constexpr (n > 1) {
+  if constexpr (n == 2 * GC_UPW) {  // the row level
     const bool upper = (lane & O) != 0;
 #pragma unroll
     for (int i = 0; i < n / 2; ++i) {
@@ -132,6 +186,9 @@ __device__ __forceinline__ void gc_reduce_level(float (&v)[N], int lane) {
       const float send = upper ? v[i] : v[i + n / 2];
       v[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);
     }
+  } else if constexpr (n > 1) {
+#pragma unroll
+    for (int i = 0; i < n / 2; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i + n / 2], O);
   } else {
     v[0] += __shfl_xor_sync(0xffffffffu, v[0], O);
   }
@@ -139,59 +196,64 @@ __device__ __forceinline__ void gc_reduce_level(float (&v)[N], int lane) {
 }
 template <int N>
 __device__ __forceinline__ void gc_reduce_scatter(float (&v)[N], int lane) {
+  static_assert(N == GC_RB * GC_UPW || N == 2 * GC_RB * GC_UPW, "gate, row and unit index bits");
   gc_reduce_level<N, 16>(v, lane);
 }
 
 // acc[r][u] = partial (this lane's slice) of sum_k vec[row0+r][k] * w[u][k], over exactly the SL
-// elements of the slice (16-byte pieces, then an 8- and a 4-byte one as SL requires)
+// elements of the slice, in pieces of GcGeom<SL>::V floats
 template <int SL>
 __device__ __forceinline__ void gc_dot(const float* __restrict__ vec, int row0, int lane,
                                        const float (&w)[GC_UPW][SL], float (&acc)[GC_RB][GC_UPW]) {
+  constexpr int V = GcGeom<SL>::V;
 #pragma unroll
   for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
     for (int u = 0; u < GC_UPW; ++u) acc[r][u] = 0.f;
-  const float* base = vec + row0 * GcGeom<SL>::ROW + lane * GcGeom<SL>::SLP;
+  const float* base = vec + row0 * GcGeom<SL>::ROW;
 #pragma unroll
-  for (int c = 0; c < SL; c += 4) {
-    const int n = SL - c < 4 ? SL - c : 4;
+  for (int c = 0; c < SL; c += V) {
 #pragma unroll
     for (int r = 0; r < GC_RB; ++r) {
-      const float* p = base + r * GcGeom<SL>::ROW + c;
-      float x[4];
-      if (n == 4) {
+      const float* p = base + r * GcGeom<SL>::ROW + GcGeom<SL>::slice_pos(lane, c);
+      float x[V];
+      if constexpr (V == 4) {
         const float4 q = *reinterpret_cast<const float4*>(p);
         x[0] = q.x; x[1] = q.y; x[2] = q.z; x[3] = q.w;
+      } else if constexpr (V == 2) {
+        const float2 q = *reinterpret_cast<const float2*>(p);
+        x[0] = q.x; x[1] = q.y;
       } else {
-        if (n >= 2) {
-          const float2 q = *reinterpret_cast<const float2*>(p);
-          x[0] = q.x; x[1] = q.y;
-        }
-        if (n == 1) x[0] = p[0];
-        if (n == 3) x[2] = p[2];
+        x[0] = p[0];
       }
 #pragma unroll
       for (int u = 0; u < GC_UPW; ++u)
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (i < n) acc[r][u] = fmaf(x[i], w[u][c + i], acc[r][u]);
+        for (int i = 0; i < V; ++i) acc[r][u] = fmaf(x[i], w[u][c + i], acc[r][u]);
     }
   }
 }
 
 // Load this lane's slice of column (or row) vectors of a weight matrix for the warp's 4
-// units: w[u][i] = W[(k0+i)*sk + unit(u)*su], zero past H or past the CTA's units.
+// units: w[u][e] = W[k*sk + (unit0 + (u ^ usw))*su] with k the hidden unit at slice position e of
+// the vector layout, zero at padding positions or past the CTA's units (usw permutes the units:
+// see gc_reduce_scatter).
 template <int SL>
 __device__ __forceinline__ void gc_load_w(float (&w)[GC_UPW][SL], const float* __restrict__ W,
-                                          int64_t sk, int64_t su, int unit0, int unit_limit, int k0, int H) {
+                                          int64_t sk, int64_t su, int unit0, int usw, int unit_limit, int lane,
+                                          int H) {
+  const int r = lane >> 2;  // UP = 4 * SL: the slice lies inside the region of CTA lane / 4
+  const int k0 = r * H / GC_CLUSTER - r * GcGeom<SL>::UP, k_end = (r + 1) * H / GC_CLUSTER;
 #pragma unroll
-  for (int u = 0; u < GC_UPW; ++u)
+  for (int e = 0; e < SL; ++e) {
+    const int k = k0 + GcGeom<SL>::slice_pos(lane, e);
+    const bool k_ok = k < k_end;
 #pragma unroll
-    for (int i = 0; i < SL; ++i) {
-      const int unit = unit0 + u, k = k0 + i;
-      const bool ok = (unit < unit_limit) && (k < H);
-      w[u][i] = ok ? W[(int64_t)k * sk + (int64_t)unit * su] : 0.f;
+    for (int u = 0; u < GC_UPW; ++u) {
+      const int unit = unit0 + (u ^ usw);
+      w[u][e] = (k_ok && unit < unit_limit) ? W[(int64_t)k * sk + (int64_t)unit * su] : 0.f;
     }
+  }
 }
 
 // Per-phase cycle counters of thread 0 of CTA 0 (diagnostics; see nm_gru_debug_profile).  The
@@ -251,10 +313,6 @@ __device__ __forceinline__ void gc_fwd_prefetch(const GcFwdArgs& a, int t, float
   cp_async_commit();
 }
 
-// Bytes of one exchanged Bc x H vector.  Recomputed from the kernel parameters where it is used, so
-// that it holds no register across the step loop (the SL = 10 instance is at the 168-register cap).
-__device__ __forceinline__ uint32_t gc_phase_bytes(const GcFwdArgs& a) { return (uint32_t)(a.Bc * a.H * 4); }
-
 template <int SL>
 __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFwdArgs a) {
   extern __shared__ __align__(16) float gc_smem[];
@@ -278,30 +336,30 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFw
   const int unit0 = ubeg + unit0_local;               // first hidden unit of this warp
   const bool warp_live = unit0 < unit_limit;
 
-  float wr[GC_UPW][SL], wu[GC_UPW][SL], wc[GC_UPW][SL];
-  gc_load_w<SL>(wr, a.Wgh, 2 * H, 1, unit0, unit_limit, lane * SL, H);
-  gc_load_w<SL>(wu, a.Wgh + H, 2 * H, 1, unit0, unit_limit, lane * SL, H);
-  gc_load_w<SL>(wc, a.Wch, H, 1, unit0, unit_limit, lane * SL, H);
-
   // The (row, unit) result this lane holds after each reduce-scatter, fixed for the kernel.
   // Phase 1: 16 values (gate, row, unit), 2 copies; phase 2: 8 values (row, unit), 4 copies.
   const int g1 = lane >> 4, r1 = (lane >> 3) & 1, u1 = (lane >> 1) & 3;
   const int r2 = (lane >> 4) & 1, u2 = (lane >> 2) & 3, copy2 = lane & 3;
-  const int copy1 = ((lane >> 4) << 1) | (lane & 1);  // 4 lanes send each r*h value (see below)
+  // the slot order gc_reduce_scatter needs: gate g1 first, units permuted by the held ones
+  float wg[2][GC_UPW][SL], wc[GC_UPW][SL];
+  gc_load_w<SL>(wg[0], a.Wgh + g1 * H, 2 * H, 1, unit0, u1, unit_limit, lane, H);
+  gc_load_w<SL>(wg[1], a.Wgh + (g1 ^ 1) * H, 2 * H, 1, unit0, u1, unit_limit, lane, H);
+  gc_load_w<SL>(wc, a.Wch, H, 1, unit0, u2, unit_limit, lane, H);
   const bool ok1 = unit0 + u1 < unit_limit, ok2 = unit0 + u2 < unit_limit;
   const int j1 = unit0 + u1, j2 = unit0 + u2;
-  const int pos1 = ok1 ? GcGeom<SL>::pos(j1) : 0, pos2 = ok2 ? GcGeom<SL>::pos(j2) : 0;
+  // the own unit in a row of every CTA; pos & ~3 is the warp's quad
+  const int pos1 = rank * GcGeom<SL>::UP + unit0_local + u1, pos2 = rank * GcGeom<SL>::UP + unit0_local + u2;
 
   if (threadIdx.x == 0) {
     gc_mbar_init(bar_h);
     gc_mbar_init(bar_h + 8);
     gc_mbar_init(bar_rh);
-    gc_mbar_arm(bar_h, gc_phase_bytes(a));
-    gc_mbar_arm(bar_h + 8, gc_phase_bytes(a));
-    gc_mbar_arm(bar_rh, gc_phase_bytes(a));
+    gc_mbar_arm(bar_h, (uint32_t)(Bc * H * 4));  // the h0 seed below comes in 4-byte messages
+    gc_mbar_arm(bar_h + 8, gc_quad_bytes(H, Bc));
+    gc_mbar_arm(bar_rh, gc_quad_bytes(H, Bc));
   }
-  // The slice padding of the vector buffers is never written: it must be 0, not stale shared
-  // memory; padding rows (and units of the prefetch that are never loaded) stay 0 as well.
+  // Positions past a CTA's units are only written as 0 (or not at all): they must be 0, not stale
+  // shared memory; padding rows (and units of the prefetch that are never loaded) stay 0 as well.
   for (int i = threadIdx.x; i < 3 * Bc * ROW; i += GC_THREADS) hbuf[i] = 0.f;
   for (int i = threadIdx.x; i < 2 * Bc * GC_MAX_UNITS * GC_XS; i += GC_THREADS) xs[i] = 0.f;
   for (int b = threadIdx.x; b < Bc; b += GC_THREADS)
@@ -314,10 +372,10 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFw
   // to h buffer 0 of every CTA
   const int t_first = a.reverse ? T - 1 : 0;
   for (int idx = threadIdx.x; idx < Bc * UW; idx += GC_THREADS) {
-    const int b = idx / UW, j = ubeg + (idx - b * UW);
+    const int b = idx / UW, ul = idx - b * UW, j = ubeg + ul;
     const float hv = (b < nrows && a.h0) ? a.h0[(int64_t)(b0 + b) * H + j] : 0.f;
     if (b < nrows) a.hprev[((int64_t)(b0 + b) * T + t_first) * H + j] = hv;
-    const uint32_t addr = gc_smem_u32(hbuf + b * ROW + GcGeom<SL>::pos(j));
+    const uint32_t addr = gc_smem_u32(hbuf + b * ROW + rank * GcGeom<SL>::UP + ul);
     for (int d = 0; d < GC_CLUSTER; ++d) gc_send(addr, bar_h, d, hv);
   }
   gc_fwd_prefetch(a, t_first, xs, b0, nrows, ubeg, UW);
@@ -333,7 +391,7 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFw
     const float* xc = xs + par * Bc * GC_MAX_UNITS * GC_XS;
 
     gc_mbar_wait(bar_h + 8 * par, (step >> 1) & 1);
-    if (threadIdx.x == 0 && step + 2 < T) gc_mbar_arm(bar_h + 8 * par, gc_phase_bytes(a));
+    if (threadIdx.x == 0 && step + 2 < T) gc_mbar_arm(bar_h + 8 * par, gc_quad_bytes(H, Bc));
     prof.lap(a.prof, 0);
     cp_async_wait_all();
     __syncthreads();  // this step's xproj is in; every warp is done with the previous step
@@ -344,60 +402,73 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFw
     // (warps past the last unit skip the loop as a whole, which keeps every shuffle convergent)
     if (warp_live) {
       for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
-        float ar[GC_RB][GC_UPW], au[GC_RB][GC_UPW];
-        gc_dot<SL>(hb, r0, lane, wr, ar);
-        gc_dot<SL>(hb, r0, lane, wu, au);
-        float v[2 * GC_RB * GC_UPW];  // index = gate*8 + row*4 + unit
+        float a0[GC_RB][GC_UPW], a1[GC_RB][GC_UPW];
+        gc_dot<SL>(hb, r0, lane, wg[0], a0);
+        gc_dot<SL>(hb, r0, lane, wg[1], a1);
+        float v[2 * GC_RB * GC_UPW];  // slot = gate*8 + row*4 + unit, gate and unit ^ the held ones
 #pragma unroll
         for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
           for (int u = 0; u < GC_UPW; ++u) {
-            v[r * GC_UPW + u] = ar[r][u];
-            v[GC_RB * GC_UPW + r * GC_UPW + u] = au[r][u];
+            v[r * GC_UPW + u] = a0[r][u];
+            v[GC_RB * GC_UPW + r * GC_UPW + u] = a1[r][u];
           }
         gc_reduce_scatter<2 * GC_RB * GC_UPW>(v, lane);
         const int b = r0 + r1, ul = unit0_local + u1;
         const float g = sigmoidf_(v[0] + xc[(b * GC_MAX_UNITS + ul) * GC_XS + g1]);
-        const float rhv = g * hb[b * ROW + pos1];
-        // lanes L and L^16 hold r and u of the same (row, unit): the u lanes help send r*h
-        // (the shuffle runs on every lane: a shuffle skipped by some lanes of its mask never completes)
-        const float rh_peer = __shfl_xor_sync(0xffffffffu, rhv, 16);
-        const float rh_send = g1 == 0 ? rhv : rh_peer;
-        if (ok1) {
-          if ((lane & 1) == 0) {
-            if (b < nrows) {
-              const int64_t row = row0 + (int64_t)b * T;
-              a.gates[row * 3 * H + g1 * H + j1] = g;
-              if (g1 == 0) a.rh[row * H + j1] = rhv;
-            }
-            if (g1 == 1) us[b * GC_MAX_UNITS + ul] = g;
+        const float rhv = ok1 ? g * hb[b * ROW + pos1] : 0.f;  // 0 in the quad's padding slots
+        // lane L < 16 sends the r*h quad of row r1 (lanes (L & 8) | 2u hold it) to CTA L & 7, before the
+        // stores that nothing in the cluster waits for
+        // (the shuffles run on every lane: a shuffle skipped by some lanes of its mask never completes)
+        float q[4];
+        gc_gather4<0x18, 2>(q, rhv);
+        if (lane < 16) gc_send4(gc_smem_u32(rhbuf + b * ROW + (pos1 & ~3)), bar_rh, lane & 7, q);
+        if (ok1 && (lane & 1) == 0) {
+          if (b < nrows) {
+            const int64_t row = row0 + (int64_t)b * T;
+            a.gates[row * 3 * H + g1 * H + j1] = g;
+            if (g1 == 0) a.rh[row * H + j1] = rhv;
           }
-          const uint32_t addr = gc_smem_u32(rhbuf + b * ROW + pos1);
-          gc_send(addr, bar_rh, 2 * copy1, rh_send);
-          gc_send(addr, bar_rh, 2 * copy1 + 1, rh_send);
+          if (g1 == 1) us[b * GC_MAX_UNITS + ul] = g;
         }
       }
       __syncwarp();
     }
     prof.lap(a.prof, 2);
     gc_mbar_wait(bar_rh, step & 1);
-    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_rh, gc_phase_bytes(a));
+    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_rh, gc_quad_bytes(H, Bc));
     prof.lap(a.prof, 3);
 
     // ---- phase 2: c = tanh(xc + rh.Wch), h' = u*h + (1-u)*c -> every CTA ----
     if (warp_live) {
       const uint32_t bar_next = bar_h + 8 * (par ^ 1);
       float* hn_buf = hbuf + (par ^ 1) * Bc * ROW;
+      // the four copies of a (row, unit) share its stores: copy 0 the candidate gate, 1 the state, 2 the raw
+      // state, 3 the next state; `out` is the copy's element for row b0, `out_step` the step between rows
+      float* out;
+      int64_t out_step = (int64_t)T * H;
+      if (copy2 == 0) {
+        out = a.gates + row0 * 3 * H + 2 * H + j2;
+        out_step = (int64_t)T * 3 * H;
+      } else if (copy2 == 1) {
+        out = a.states + row0 * H + j2;
+      } else if (copy2 == 2) {
+        out = a.raw_states ? a.raw_states + row0 * H + j2 : nullptr;
+      } else if (last) {
+        out = a.final_state + (int64_t)b0 * H + j2;
+        out_step = H;
+      } else {
+        out = a.hprev + ((int64_t)b0 * T + t_next) * H + j2;
+      }
       for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
         float ac[GC_RB][GC_UPW];
         gc_dot<SL>(rhbuf, r0, lane, wc, ac);
-        float v[GC_RB * GC_UPW];  // index = row*4 + unit
+        float v[GC_RB * GC_UPW];  // slot = row*4 + unit, unit ^ the held one
 #pragma unroll
         for (int r = 0; r < GC_RB; ++r)
 #pragma unroll
           for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = ac[r][u];
         gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
-        if (!ok2) continue;
         const int b = r0 + r2, ul = unit0_local + u2;
         const float* xd = xc + (b * GC_MAX_UNITS + ul) * GC_XS;
         const float c = tanhf(v[0] + xd[2]);
@@ -408,18 +479,14 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_fwd_cluster_kernel(GcFw
         const float raw = live ? hn : 0.f;
         // the decoder feeds the DROPPED-OUT cell output back as the next state
         if (a.drop_mask && live) hn *= xd[3];
-        if (b < nrows) {  // the four copies share the stores
-          const int64_t row = row0 + (int64_t)b * T;
-          if (copy2 == 0) a.gates[row * 3 * H + 2 * H + j2] = c;
-          else if (copy2 == 1) a.states[row * H + j2] = live ? hn : 0.f;
-          else if (copy2 == 2) { if (a.raw_states) a.raw_states[row * H + j2] = raw; }
-          else if (last) a.final_state[(int64_t)(b0 + b) * H + j2] = hn;
-          else a.hprev[((int64_t)(b0 + b) * T + t_next) * H + j2] = hn;
+        if (!last) {  // lane L with bit 3 clear sends the h' quad of row r2 (lanes (L & 16) | 4u) to CTA L & 7
+          float q[4];
+          gc_gather4<0x10, 4>(q, ok2 ? hn : 0.f);
+          if ((lane & 8) == 0) gc_send4(gc_smem_u32(hn_buf + b * ROW + (pos2 & ~3)), bar_next, lane & 7, q);
         }
-        if (!last) {
-          const uint32_t addr = gc_smem_u32(hn_buf + b * ROW + pos2);
-          gc_send(addr, bar_next, 2 * copy2, hn);
-          gc_send(addr, bar_next, 2 * copy2 + 1, hn);
+        if (ok2 && b < nrows && out) {
+          const float val = copy2 == 0 ? c : copy2 == 1 ? (live ? hn : 0.f) : copy2 == 2 ? raw : hn;
+          out[b * out_step] = val;
         }
       }
     }
@@ -501,7 +568,6 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
   float* pf = dhp + Bc * GC_MAX_UNITS;          // [2][Bc][GC_MAX_UNITS][GC_PF] by step parity
   int* lens = reinterpret_cast<int*>(pf + 2 * Bc * GC_MAX_UNITS * GC_PF);  // [Bc]; 0 for padding rows
   const uint32_t bar_a = gc_smem_u32(gc_smem), bar_b = bar_a + 16;     // bar_a + 8*parity: dz_c + dz_u
-  const uint32_t bytes_a = (uint32_t)(2 * Bc * H * 4), bytes_b = (uint32_t)(Bc * H * 4);
 
   const int rank = (int)cluster_rank();
   const int ubeg = rank * H / GC_CLUSTER;      // first hidden unit of this CTA
@@ -514,17 +580,17 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
   const int unit0 = ubeg + unit0_local;        // first OUTPUT unit i of this warp
   const bool warp_live = unit0 < unit_limit;
 
-  // rows i of Wch / Wgh restricted to this lane's slice of the reduction index j
-  float w1[GC_UPW][SL], w2r[GC_UPW][SL], w2u[GC_UPW][SL];
-  gc_load_w<SL>(w1, a.Wch, 1, H, unit0, unit_limit, lane * SL, H);
-  gc_load_w<SL>(w2r, a.Wgh, 1, 2 * H, unit0, unit_limit, lane * SL, H);
-  gc_load_w<SL>(w2u, a.Wgh + H, 1, 2 * H, unit0, unit_limit, lane * SL, H);
-
   // the (row, unit) this lane holds after a reduce-scatter of 8 values, and its copy index
   const int rr_ = (lane >> 4) & 1, uq = (lane >> 2) & 3, copy = lane & 3;
+  // rows i of Wch / Wgh restricted to this lane's slice of the reduction index j, the units in the
+  // slot order of gc_reduce_scatter
+  float w1[GC_UPW][SL], w2r[GC_UPW][SL], w2u[GC_UPW][SL];
+  gc_load_w<SL>(w1, a.Wch, 1, H, unit0, uq, unit_limit, lane, H);
+  gc_load_w<SL>(w2r, a.Wgh, 1, 2 * H, unit0, uq, unit_limit, lane, H);
+  gc_load_w<SL>(w2u, a.Wgh + H, 1, 2 * H, unit0, uq, unit_limit, lane, H);
   const bool ok = unit0 + uq < unit_limit;
   const int ji = unit0 + uq, ul = unit0_local + uq;
-  const int pos = ok ? GcGeom<SL>::pos(ji) : 0;
+  const int quad = rank * GcGeom<SL>::UP + unit0_local;  // the warp's units in a row of every CTA
   // time of the k-th step processed
   auto time_of = [reverse = a.reverse, T](int k) { return reverse ? k : T - 1 - k; };
 
@@ -532,9 +598,9 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
     gc_mbar_init(bar_a);
     gc_mbar_init(bar_a + 8);
     gc_mbar_init(bar_b);
-    gc_mbar_arm(bar_a, bytes_a);
-    gc_mbar_arm(bar_a + 8, bytes_a);
-    gc_mbar_arm(bar_b, bytes_b);
+    gc_mbar_arm(bar_a, (uint32_t)(2 * Bc * H * 4));  // the E1 seed below comes in 4-byte messages
+    gc_mbar_arm(bar_a + 8, 2 * gc_quad_bytes(H, Bc));
+    gc_mbar_arm(bar_b, gc_quad_bytes(H, Bc));
   }
   for (int i = threadIdx.x; i < 4 * Bc * ROW; i += GC_THREADS) vc[i] = 0.f;  // vc, vu, vr; see fwd
   for (int i = threadIdx.x; i < 2 * Bc * GC_MAX_UNITS * GC_PF; i += GC_THREADS) pf[i] = 0.f;
@@ -560,7 +626,7 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
         a.dxproj[row * 3 * H + H + j] = zu;
         a.dxproj[row * 3 * H + 2 * H + j] = zc;
       }
-      const int p = GcGeom<SL>::pos(j);
+      const int p = rank * GcGeom<SL>::UP + u;
       const uint32_t ac = gc_smem_u32(vc + b * ROW + p), au = gc_smem_u32(vu + b * ROW + p);
       for (int d = 0; d < GC_CLUSTER; ++d) {
         gc_send(ac, bar_a, d, zc);
@@ -579,7 +645,7 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
     float* pfn = pf + (par ^ 1) * Bc * GC_MAX_UNITS * GC_PF;
 
     gc_mbar_wait(bar_a + 8 * par, (k >> 1) & 1);
-    if (threadIdx.x == 0 && k + 2 < T) gc_mbar_arm(bar_a + 8 * par, bytes_a);
+    if (threadIdx.x == 0 && k + 2 < T) gc_mbar_arm(bar_a + 8 * par, 2 * gc_quad_bytes(H, Bc));
     prof.lap(a.prof, 0);
     __syncthreads();  // every warp is done with the previous step (and its prefetch slot)
     if (!last) gc_bwd_prefetch(a, time_of(k + 1), pfn, lens, b0, ubeg, UW);
@@ -596,26 +662,26 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
 #pragma unroll
           for (int u = 0; u < GC_UPW; ++u) v[r * GC_UPW + u] = acc[r][u];
         gc_reduce_scatter<GC_RB * GC_UPW>(v, lane);
-        if (!ok) continue;
         const int b = r0 + rr_;
         const float drh = v[0];
         const bool live = t < lens[b];
         const float* s = pfc + (b * GC_MAX_UNITS + ul) * GC_PF;
         const float rg = s[0], hv = s[3];
-        const float zr = live ? drh * hv * rg * (1.f - rg) : 0.f;
-        if (copy == 0) {
+        const float zr = (ok && live) ? drh * hv * rg * (1.f - rg) : 0.f;  // 0 in the quad's padding slots
+        if (ok && copy == 0) {
           if (b < nrows) a.dxproj[(row0 + (int64_t)b * T) * 3 * H + ji] = zr;
           if (live) dhp[b * GC_MAX_UNITS + ul] += drh * rg;
         }
-        const uint32_t addr = gc_smem_u32(vr + b * ROW + pos);
-        gc_send(addr, bar_b, 2 * copy, zr);
-        gc_send(addr, bar_b, 2 * copy + 1, zr);
+        // lane L with bit 3 clear sends the dz_r quad of row rr_ (lanes (L & 16) | 4u) to CTA L & 7
+        float q[4];
+        gc_gather4<0x10, 4>(q, zr);
+        if ((lane & 8) == 0) gc_send4(gc_smem_u32(vr + b * ROW + quad), bar_b, lane & 7, q);
       }
       __syncwarp();
     }
     prof.lap(a.prof, 2);
     gc_mbar_wait(bar_b, k & 1);
-    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_b, bytes_b);
+    if (threadIdx.x == 0 && !last) gc_mbar_arm(bar_b, gc_quad_bytes(H, Bc));
     prof.lap(a.prof, 3);
     cp_async_wait_all();
     __syncthreads();  // the next step's prefetch is in
@@ -624,6 +690,7 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
     // ---- G2: dcarry = dhp + [dz_r, dz_u] . Wgh^T, then E1 of the next step -> dz_c, dz_u ----
     if (warp_live) {
       const float* vuc = vu + par * Bc * ROW;
+      float* const send_buf = (lane & 2) ? vu + (par ^ 1) * Bc * ROW : vc;  // dz_u or dz_c (see below)
       const int tn = last ? t : time_of(k + 1);
       for (int r0 = 0; r0 < Bc; r0 += GC_RB) {
         float accr[GC_RB][GC_UPW], accu[GC_RB][GC_UPW];
@@ -638,26 +705,25 @@ __global__ void __launch_bounds__(GC_THREADS, 1) gru_seq_bwd_cluster_kernel(GcBw
         const int b = r0 + rr_;
         const float dcarry = ok ? dhp[b * GC_MAX_UNITS + ul] + v[0] : 0.f;
         __syncwarp();  // every copy has read dhp before copy 0 replaces it
-        if (!ok) continue;
         if (last) {
-          if (a.dh0 && copy == 0 && b < nrows) a.dh0[(int64_t)(b0 + b) * H + ji] = dcarry;
+          if (ok && a.dh0 && copy == 0 && b < nrows) a.dh0[(int64_t)(b0 + b) * H + ji] = dcarry;
           continue;
         }
         float zc, zu;
         const float d = gc_bwd_e1(a, pfn + (b * GC_MAX_UNITS + ul) * GC_PF, dcarry, tn < lens[b], zc, zu);
-        if (b < nrows) {
-          const int64_t row = (int64_t)(b0 + b) * T + tn;
-          if (copy == 1) a.dxproj[row * 3 * H + H + ji] = zu;
-          else if (copy == 2) a.dxproj[row * 3 * H + 2 * H + ji] = zc;
+        if (ok) {
+          if (b < nrows) {
+            const int64_t row = (int64_t)(b0 + b) * T + tn;
+            if (copy == 1) a.dxproj[row * 3 * H + H + ji] = zu;
+            else if (copy == 2) a.dxproj[row * 3 * H + 2 * H + ji] = zc;
+          }
+          if (copy == 0) dhp[b * GC_MAX_UNITS + ul] = d;
         }
-        if (copy == 0) dhp[b * GC_MAX_UNITS + ul] = d;
-        const uint32_t ac = gc_smem_u32(vc + b * ROW + pos);
-        const uint32_t au = gc_smem_u32(vu + ((par ^ 1) * Bc + b) * ROW + pos);
-        const uint32_t bar_next = bar_a + 8 * (par ^ 1);
-        gc_send(ac, bar_next, 2 * copy, zc);
-        gc_send(ac, bar_next, 2 * copy + 1, zc);
-        gc_send(au, bar_next, 2 * copy, zu);
-        gc_send(au, bar_next, 2 * copy + 1, zu);
+        // copies 0, 1 pass on dz_c and copies 2, 3 dz_u; lane L sends the dz_c (bit 1 clear) or dz_u quad
+        // of row rr_ (lanes (L & 18) | 4u) to CTA ((L >> 1) & 6) | (L & 1): all 32 lanes one message each
+        float q[4];
+        gc_gather4<0x12, 4>(q, ok ? (copy & 2 ? zu : zc) : 0.f);
+        gc_send4(gc_smem_u32(send_buf + b * ROW + quad), bar_a + 8 * (par ^ 1), ((lane >> 1) & 6) | (lane & 1), q);
       }
     }
     prof.lap(a.prof, 5);
