@@ -7,7 +7,7 @@
  * (neuralmonkey/tf_manager.py:179-180).  Every entry point below replaces the
  * TF op group named in its comment (reference file:line), and is what a
  * ctypes binding inside the reference's ModelPart classes would call
- * (see INTEGRATION.md).  73 entry points.
+ * (see INTEGRATION.md).  89 entry points.
  *
  * Conventions
  *   - plain pointers + int64_t sizes; no torch / C++ types cross the ABI;
@@ -678,6 +678,37 @@ int64_t nm_glu_conv1d_wgrad_workspace(int64_t B, int64_t T, int64_t F, int64_t k
 int nm_glu_conv1d_wgrad(const float* x, const float* dz, float* dw, float* db, float* workspace,
                         int64_t workspace_floats, int64_t B, int64_t T, int64_t F, int64_t k, int backend,
                         void* stream);
+
+/* ---- K20: speech features ---------------------------------------------------------------------------
+ * Replace python_speech_features 0.6.1's mfcc / fbank / logfbank / ssc and delta, which the reference's
+ * processors/speech.py:43-62 calls once per utterance (SpeechFeaturesPreprocessor).  All arithmetic is fp64.
+ * nm_speech_features: signal [samples] f64 is pre-emphasised (y[0] = x[0], y[n] = x[n] - preemph*x[n-1]), cut into
+ *   `frames` frames of frame_len samples every frame_step samples (zeros past the end), each multiplied by window
+ *   [frame_len] f64, truncated or zero-padded to nfft (a power of two, 2..8192); pspec = |rfft|^2 / nfft over the
+ *   nfft/2+1 bins.  fbank [nfilt, nfft/2+1] f64 is the filterbank matrix; filter j reads only the bins
+ *   [fb_first[j], fb_last[j]) (i32), which must hold all its nonzero entries; nfilt <= 1024.  Per frame, into the
+ *   first `width` columns of row f of out (row stride out_stride):
+ *     NM_SPEECH_FBANK     pspec . fbank^T, zeros replaced by DBL_EPSILON (width = nfilt);
+ *     NM_SPEECH_LOGFBANK  its log;
+ *     NM_SPEECH_MFCC      DCT-II (ortho) of the log, the first width = min(numcep, nfilt) coefficients, times
+ *                         1 + (ceplifter/2) sin(pi n / ceplifter) when ceplifter > 0, column 0 replaced by
+ *                         log(sum pspec) (zero energy -> DBL_EPSILON) when append_energy != 0;
+ *     NM_SPEECH_SSC       (pspec' * R) . fbank^T / (pspec' . fbank^T) with pspec' = pspec, zeros -> DBL_EPSILON,
+ *                         R = linspace(1, rate/2, nfft/2+1); an all-zero filter gives NaN (width = nfilt).
+ * nm_speech_deltas: columns [(block+1)*width, (block+2)*width) of out [frames, out_stride] f64 become the deltas of
+ *   columns [block*width, (block+1)*width): d[t] = sum_{n=-N..N} n x[clamp(t+n, 0, frames-1)] / (2 sum_{n=1..N} n^2),
+ *   N = window (1..1024). */
+#define NM_SPEECH_MFCC 0
+#define NM_SPEECH_FBANK 1
+#define NM_SPEECH_LOGFBANK 2
+#define NM_SPEECH_SSC 3
+int nm_speech_features(const double* signal, int64_t samples, const double* window, int64_t frame_len,
+                       int64_t frame_step, int64_t nfft, double preemph, const double* fbank,
+                       const int32_t* fb_first, const int32_t* fb_last, int64_t nfilt, int kind, int64_t numcep,
+                       double ceplifter, int append_energy, double rate, double* out, int64_t frames,
+                       int64_t out_stride, void* stream);
+int nm_speech_deltas(double* out, int64_t frames, int64_t width, int64_t out_stride, int64_t block, int64_t window,
+                     void* stream);
 
 #ifdef __cplusplus
 }

@@ -23,7 +23,7 @@ def parse_header(path: str = HEADER_PATH) -> Dict[str, str]:
     """Derive ctypes signatures from the C header so the two cannot drift.
 
     Returns {function name: (restype code, argument codes)} with codes
-    p = pointer, i = int, l = int64_t, f = float, v = void (no arguments).
+    p = pointer, i = int, l = int64_t, f = float, d = double, v = void (no arguments).
     """
     import re
     text = open(path, encoding="utf-8").read()
@@ -42,6 +42,8 @@ def parse_header(path: str = HEADER_PATH) -> Dict[str, str]:
                     codes += "l"
                 elif arg.startswith("float"):
                     codes += "f"
+                elif arg.startswith("double"):
+                    codes += "d"
                 elif arg.startswith("int"):
                     codes += "i"
                 else:
@@ -52,7 +54,7 @@ def parse_header(path: str = HEADER_PATH) -> Dict[str, str]:
 
 
 _CTYPES = {"p": ctypes.c_void_p, "i": ctypes.c_int, "l": ctypes.c_int64,
-           "f": ctypes.c_float}
+           "f": ctypes.c_float, "d": ctypes.c_double}
 
 
 class NMB200Error(RuntimeError):

@@ -1679,3 +1679,46 @@ def squared_error(pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         raise ValueError("squared_error: predictions [B, dim] and targets [B], got {} and {}".format(
             tuple(pred.shape), tuple(target.shape)))
     return _SquaredError.apply(pred, target)
+
+
+# ---------------------------------------------------------------------------
+# K20 speech features
+# ---------------------------------------------------------------------------
+SPEECH_KINDS = {"mfcc": 0, "fbank": 1, "logfbank": 2, "ssc": 3}   # NM_SPEECH_* of include/nmb200.h
+
+
+def speech_frame_count(samples: int, frame_len: int, frame_step: int) -> int:
+    """Frames of python_speech_features' framesig: one when the signal fits in a frame, else enough frames at
+    `frame_step` to cover it, the last one zero-padded."""
+    if samples <= frame_len:
+        return 1
+    return 1 + -(-(samples - frame_len) // frame_step)
+
+
+def speech_features(signal: torch.Tensor, window: torch.Tensor, frame_step: int, nfft: int, preemph: float,
+                    fbank: torch.Tensor, fb_first: torch.Tensor, fb_last: torch.Tensor, kind: str, rate: float,
+                    numcep: int = 13, ceplifter: float = 0.0, append_energy: bool = False, delta_order: int = 0,
+                    delta_window: int = 2) -> torch.Tensor:
+    """Speech features of one utterance (processors/speech.py): the `kind` features of python_speech_features
+    0.6.1 over the fp64 device signal [samples], framed by the fp64 window [frame_len] every `frame_step` samples,
+    followed by `delta_order` orders of deltas.  fbank [nfilt, nfft/2+1] fp64 is the filterbank, fb_first /
+    fb_last [nfilt] int32 its nonzero bin ranges.  Returns [frames, width * (1 + delta_order)] fp64."""
+    for name, t, dtype in (("signal", signal, torch.float64), ("window", window, torch.float64),
+                           ("fbank", fbank, torch.float64), ("fb_first", fb_first, torch.int32),
+                           ("fb_last", fb_last, torch.int32)):
+        if t.dtype != dtype or not t.is_contiguous():
+            raise ValueError("speech_features: {} must be a contiguous {} tensor".format(name, dtype))
+    nfilt = fbank.shape[0]
+    if fbank.dim() != 2 or fbank.shape[1] != nfft // 2 + 1 or fb_first.shape != (nfilt,) or fb_last.shape != (nfilt,):
+        raise ValueError("speech_features: filterbank [nfilt, nfft/2+1] and bin ranges [nfilt] expected")
+    frame_len = window.numel()
+    frames = speech_frame_count(signal.numel(), frame_len, frame_step)
+    width = min(numcep, nfilt) if kind == "mfcc" else nfilt
+    stride = width * (1 + delta_order)
+    out = torch.empty(frames, stride, device=signal.device, dtype=torch.float64)
+    call("nm_speech_features", ptr(signal), signal.numel(), ptr(window), frame_len, frame_step, nfft, float(preemph),
+         ptr(fbank), ptr(fb_first), ptr(fb_last), nfilt, SPEECH_KINDS[kind], numcep, float(ceplifter),
+         int(append_energy), float(rate), ptr(out), frames, stride, lib.stream())
+    for block in range(delta_order):
+        call("nm_speech_deltas", ptr(out), frames, width, stride, block, delta_window, lib.stream())
+    return out
