@@ -219,6 +219,45 @@ int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask,
                     float* de_work, int64_t B, int64_t Tx, int64_t NQ, int64_t A,
                     int64_t C, void* stream);
 
+/* ---- Joint multi-source attention --------------------------------------------
+ * Replaces FlatMultiAttention.attention (attention/combination.py:240-321) and
+ * HierarchicalMultiAttention.attention (:394-463) for NQ query steps at once:
+ *     e[b,q,t]    = sum_a v[a]*tanh(keys[b,t,a] + qproj[b,q,a]) + seg_bias[seg(t)]
+ *     e[b,q,Tx+j] = sum_a v[a]*tanh(ckeys[b,q,j,a] + qproj[b,q,a]) + cand_bias[j]
+ *     p = softmax over all L = Tx + J positions
+ *     mask given: w = p*m / (sum p*m + 1e-8), m = mask[b,t] (t < Tx), 1 (candidates)
+ *     mask NULL:  w = p
+ *     ctx[b,q] = sum_t w[b,q,t]*values[b,t,:] + sum_j w[b,q,Tx+j]*cvalues[b,q,j,:]
+ * keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] (may be NULL), seg_ends: HOST array
+ * of S cumulative segment ends (the last is Tx; S = 0 iff Tx = 0; S <= 8),
+ * seg_bias [S], ckeys [B,NQ,J,A], cvalues [B,NQ,J,C], cand_bias [J], qproj
+ * [B,NQ,A], v [A].  Tx = 0 or J = 0 is allowed (not both); the pointers of an
+ * empty part may be NULL.  Outputs: energies [B,NQ,L] (saved for backward; may
+ * be NULL), weights [B,NQ,L], ctx [B,NQ,C].  fp32 throughout. */
+int nm_joint_attention_fwd(const float* keys, const float* values,
+                           const float* mask, const int64_t* seg_ends,
+                           const float* seg_bias, const float* ckeys,
+                           const float* cvalues, const float* cand_bias,
+                           const float* qproj, const float* v, float* energies,
+                           float* weights, float* ctx, int64_t B, int64_t Tx,
+                           int64_t S, int64_t J, int64_t NQ, int64_t A,
+                           int64_t C, void* stream);
+/* Backward.  dkeys, dvalues, dqproj, dckeys, dcvalues are overwritten; dv [A],
+ * dseg_bias [S] and dcand_bias [J] are accumulated into.  The gradient reaches
+ * masked energies too.  No atomics: repeated calls give identical bits.  work is
+ * scratch of B*NQ*(Tx+J) + B*A + B*(S+J) floats. */
+int nm_joint_attention_bwd(const float* keys, const float* values,
+                           const float* mask, const int64_t* seg_ends,
+                           const float* ckeys, const float* cvalues,
+                           const float* qproj, const float* v,
+                           const float* energies, const float* weights,
+                           const float* dctx, float* dkeys, float* dvalues,
+                           float* dqproj, float* dckeys, float* dcvalues,
+                           float* dv, float* dseg_bias, float* dcand_bias,
+                           float* work, int64_t B, int64_t Tx, int64_t S,
+                           int64_t J, int64_t NQ, int64_t A, int64_t C,
+                           void* stream);
+
 /* ---- K5/K6: vocabulary projection loss ---------------------------------------
  * Replaces log_softmax + tf.contrib.seq2seq.sequence_loss
  * (decoders/autoregressive.py:288-316) and the greedy argmax (:446-480).

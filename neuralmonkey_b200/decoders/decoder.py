@@ -187,6 +187,25 @@ class Decoder(AutoregressiveDecoder):
             init = init.unsqueeze(0).expand(self.batch_size, -1).contiguous()
         return init
 
+    @staticmethod
+    def _attend_sequence(att, queries, prev_outputs, inputs):
+        """att.attention_sequence over queries [B, NQ, rnn]; attentions that declare `wants_sentinel_inputs`
+        (attention.combination) also get each query step's previous cell output and embedded input
+        [B, NQ, .], which `next_state` hands to `attention()` at run time."""
+        if getattr(att, "wants_sentinel_inputs", False):
+            return att.attention_sequence(queries, prev_outputs, inputs)
+        return att.attention_sequence(queries)
+
+    def _step_attend(self, prev_output, rnn_input):
+        """`attend(att, query)` of one teacher-forced or differentiable step: prev_output is what the step
+        received (the (c, h) pair of an LSTM), rnn_input the step's embedded input."""
+        prev_h = prev_output[1] if isinstance(prev_output, tuple) else prev_output
+
+        def attend(att, query):
+            ctx, w = self._attend_sequence(att, query.unsqueeze(1), prev_h.unsqueeze(1), rnn_input.unsqueeze(1))
+            return ctx[:, 0], w
+        return attend
+
     # -- variants: one step of decoder.py:279-358 with the context inside the recurrence ---------
     def _variant_step(self, rnn_input: torch.Tensor, prev_output: torch.Tensor, attend):
         """(output, dropped cell output, dropped contexts, attention results) of one step.
@@ -224,13 +243,8 @@ class Decoder(AutoregressiveDecoder):
         if self._rnn_cell_str == "LSTM":
             prev = (prev, prev)
         outputs, cells, weights = [], [], [[] for _ in self.attentions]
-
-        def attend(att, query):
-            ctx, w = att.attention_sequence(query.unsqueeze(1))    # one query per sentence: NQ = 1
-            return ctx[:, 0], w
-
-        for t in range(fed.shape[1]):
-            out, prev, _ctx, attended = self._variant_step(emb[:, t], prev, attend)
+        for t in range(fed.shape[1]):       # one query per sentence and step: NQ = 1
+            out, prev, _ctx, attended = self._variant_step(emb[:, t], prev, self._step_attend(prev, emb[:, t]))
             outputs.append(out)
             cells.append(prev[1] if isinstance(prev, tuple) else prev)
             for hist, (_c, w) in zip(weights, attended):
@@ -252,9 +266,13 @@ class Decoder(AutoregressiveDecoder):
                             emb.device)
         dropped, _final, raw = ops.gru_layer(emb, *gru_cell_tensors(self, self._CELL_SCOPE),
                                              h0=self.initial_state, drop_mask=mask)
+        # the previous output each step hands to the attention: the initial state, then the dropped cell outputs
+        prev_outputs = None
+        if any(getattr(att, "wants_sentinel_inputs", False) for att in self.attentions):
+            prev_outputs = torch.cat([self.initial_state.unsqueeze(1), dropped[:, :-1]], 1)
         contexts, weights = [], []
         for att in self.attentions:
-            ctx, w = att.attention_sequence(raw)           # queries = cell outputs BEFORE dropout
+            ctx, w = self._attend_sequence(att, raw, prev_outputs, emb)   # queries = cell outputs BEFORE dropout
             contexts.append(dropout(ctx, self.dropout_keep_prob, self.train_mode))
             weights.append(w)
         out = self.output_projection(self, dropped, emb, contexts, self.train_mode)  # [B,T,O]
@@ -295,13 +313,10 @@ class Decoder(AutoregressiveDecoder):
         if self._rnn_cell_str == "LSTM":
             prev = (prev, prev)
 
-        def attend(att, query):
-            ctx, w = att.attention_sequence(query.unsqueeze(1))
-            return ctx[:, 0], w
-
         states, chosen, argmaxes, masks = [], [], [], []
         for step in range(self.max_output_len):
-            out, prev, _ctx, _attended = self._variant_step(self.embed_input_symbols(symbols), prev, attend)
+            emb = self.embed_input_symbols(symbols)
+            out, prev, _ctx, _attended = self._variant_step(emb, prev, self._step_attend(prev, emb))
             with torch.no_grad():
                 logits, _lse, argmax = self.state_to_logits(out.detach(), keep_logits=sample)
                 if sample:

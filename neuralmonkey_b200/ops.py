@@ -7,7 +7,9 @@ may carry an ``nm_grad`` attribute (a view into the flat gradient arena of
 weight gradients straight into that arena (GEMM epilogue ``beta = 1``) and return
 ``None`` to autograd, so no torch kernels run on the weight-gradient path.
 """
-from typing import Optional, Tuple
+from typing import Optional, Sequence, Tuple
+
+import ctypes
 
 import torch
 
@@ -688,6 +690,81 @@ def bahdanau_attention(keys: torch.Tensor, values: torch.Tensor, mask: Optional[
     keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] or None, qproj [B,NQ,A], v [A], bias [1].
     Returns (contexts [B,NQ,C], weights [B,NQ,Tx])."""
     return _Bahdanau.apply(keys, values, mask, qproj, v, bias)
+
+
+# ---------------------------------------------------------------------------
+# Joint multi-source attention (attention.combination)
+# ---------------------------------------------------------------------------
+class _JointAttention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keys, values, mask, seg_ends, seg_bias, ckeys, cvalues, cand_bias, qproj, v):
+        bsz, nq, a = qproj.shape
+        tx = keys.size(1) if keys is not None else 0
+        j = ckeys.size(2) if ckeys is not None else 0
+        c = values.size(2) if values is not None else cvalues.size(3)
+        keys, values, ckeys, cvalues = (t.contiguous() if t is not None else None
+                                        for t in (keys, values, ckeys, cvalues))
+        qproj = qproj.contiguous()
+        mask_c = mask.contiguous() if mask is not None else None
+        ends = (ctypes.c_int64 * max(len(seg_ends), 1))(*seg_ends)
+        dev = qproj.device
+        energies = torch.empty(bsz, nq, tx + j, device=dev, dtype=torch.float32)
+        weights = torch.empty(bsz, nq, tx + j, device=dev, dtype=torch.float32)
+        ctxv = torch.empty(bsz, nq, c, device=dev, dtype=torch.float32)
+        call("nm_joint_attention_fwd", ptr(keys), ptr(values), ptr(mask_c), ctypes.addressof(ends), ptr(seg_bias),
+             ptr(ckeys), ptr(cvalues), ptr(cand_bias), ptr(qproj), ptr(v), ptr(energies), ptr(weights), ptr(ctxv),
+             bsz, tx, len(seg_ends), j, nq, a, c, lib.stream())
+        ctx.save_for_backward(keys, values, mask_c, ckeys, cvalues, qproj, v, energies, weights)
+        ctx.seg_ends = tuple(seg_ends)
+        ctx.sinks = (_sink(v), _sink(seg_bias) if seg_bias is not None else None,
+                     _sink(cand_bias) if cand_bias is not None else None)
+        ctx.bias_shapes = (None if seg_bias is None else seg_bias.shape, None if cand_bias is None else cand_bias.shape)
+        ctx.mark_non_differentiable(weights)
+        return ctxv, weights
+
+    @staticmethod
+    def backward(ctx, dctx, _dweights):
+        keys, values, mask, ckeys, cvalues, qproj, v, energies, weights = ctx.saved_tensors
+        bsz, nq, a = qproj.shape
+        tx, j, c = energies.size(2) - (ckeys.size(2) if ckeys is not None else 0), \
+            (ckeys.size(2) if ckeys is not None else 0), dctx.size(2)
+        dev = qproj.device
+        dctx = dctx.contiguous()
+        ends = (ctypes.c_int64 * max(len(ctx.seg_ends), 1))(*ctx.seg_ends)
+        dkeys = torch.empty_like(keys) if keys is not None else None
+        dvalues = torch.empty_like(values) if values is not None else None
+        dckeys = torch.empty_like(ckeys) if ckeys is not None else None
+        dcvalues = torch.empty_like(cvalues) if cvalues is not None else None
+        dq = torch.empty_like(qproj)
+        sv, ss, sc = ctx.sinks
+        seg_shape, cand_shape = ctx.bias_shapes
+        dv = sv if sv is not None else torch.zeros(a, device=dev, dtype=torch.float32)
+        dseg = ss if ss is not None else (torch.zeros(seg_shape, device=dev, dtype=torch.float32)
+                                          if seg_shape is not None else None)
+        dcand = sc if sc is not None else (torch.zeros(cand_shape, device=dev, dtype=torch.float32)
+                                           if cand_shape is not None else None)
+        work = torch.empty(bsz * nq * (tx + j) + bsz * a + bsz * (len(ctx.seg_ends) + j), device=dev,
+                           dtype=torch.float32)
+        call("nm_joint_attention_bwd", ptr(keys), ptr(values), ptr(mask), ctypes.addressof(ends), ptr(ckeys),
+             ptr(cvalues), ptr(qproj), ptr(v), ptr(energies), ptr(weights), ptr(dctx), ptr(dkeys), ptr(dvalues),
+             ptr(dq), ptr(dckeys), ptr(dcvalues), ptr(dv), ptr(dseg), ptr(dcand), ptr(work),
+             bsz, tx, len(ctx.seg_ends), j, nq, a, c, lib.stream())
+        return (dkeys, dvalues, None, None, None if ss is not None else dseg, dckeys, dcvalues,
+                None if sc is not None else dcand, dq, None if sv is not None else dv)
+
+
+def joint_attention(keys: Optional[torch.Tensor], values: Optional[torch.Tensor], mask: Optional[torch.Tensor],
+                    seg_ends: Sequence[int], seg_bias: Optional[torch.Tensor], ckeys: Optional[torch.Tensor],
+                    cvalues: Optional[torch.Tensor], cand_bias: Optional[torch.Tensor], qproj: torch.Tensor,
+                    v: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """One softmax over shared keys in segments and per-query candidates (attention/combination.py:240-321 flat,
+    :394-463 hierarchical) for all query steps at once.
+
+    keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] or None, seg_ends: the cumulative ends of the S segments of Tx,
+    seg_bias [S] (one energy bias per segment), ckeys [B,NQ,J,A], cvalues [B,NQ,J,C], cand_bias [J],
+    qproj [B,NQ,A], v [A].  With Tx = 0 the shared arguments are None (and seg_ends empty); with J = 0 the
+    candidate ones.  Returns (contexts [B,NQ,C], weights [B,NQ,Tx+J])."""
+    return _JointAttention.apply(keys, values, mask, list(seg_ends), seg_bias, ckeys, cvalues, cand_bias, qproj, v)
 
 
 # ---------------------------------------------------------------------------
