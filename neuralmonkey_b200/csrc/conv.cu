@@ -83,10 +83,13 @@ conv3x3_kernel(const float* __restrict__ x, const float* __restrict__ w, const f
 }
 
 // im2col for the tensor-core path: cols[m][tap*Cin + c] = x[n, y+dy, x+dx, c] (zero outside the
-// image), row pitch `ldc` floats.  One thread per (pixel, tap, 4-channel group).
+// image), row pitch `ldc` floats.  One thread per (pixel, tap, 4-channel group); the group moves as one
+// float4 when Cin, ldc and both pointers keep it 16-byte aligned.
 __global__ void im2col3x3_kernel(const float* __restrict__ x, float* __restrict__ cols, int64_t NB, int H,
                                  int W, int Cin, int64_t ldc) {
   const int groups = (Cin + 3) / 4;
+  const bool vec = (Cin & 3) == 0 && (ldc & 3) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(cols)) & 15) == 0;
   const int64_t total = NB * H * W * 9 * groups;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
@@ -101,7 +104,7 @@ __global__ void im2col3x3_kernel(const float* __restrict__ x, float* __restrict_
     const bool inside = yy >= 0 && yy < H && xx >= 0 && xx < W;
     const float* src = x + ((n * H + yy) * W + xx) * Cin + 4 * g;
     float* dst = cols + m * ldc + tap * Cin + 4 * g;
-    if ((Cin & 3) == 0) {
+    if (vec) {
       const float4 v = inside ? *reinterpret_cast<const float4*>(src) : make_float4(0.f, 0.f, 0.f, 0.f);
       *reinterpret_cast<float4*>(dst) = v;
     } else {
