@@ -448,7 +448,9 @@ int nm_mha_tc_bwd(const float* q, const float* k, const float* v, const float* k
 /* ---- K12: VGG convolution stack primitives (forward only; the encoder is frozen,
  * encoders/imagenet_encoder.py:212,234) -----------------------------------------
  * NHWC fp32; 3x3, stride 1, SAME padding, + bias + ReLU (slim vgg_arg_scope);
- * w is [3,3,Cin,Cout] (HWIO, the slim checkpoint layout). */
+ * w is [3,3,Cin,Cout] (HWIO, the slim checkpoint layout).  Exact fp32 on the CUDA cores: the NM_GEMM_SIMT
+ * forward of nm_conv2d_fwd (csrc/conv_igemm.cuh).  Any batch whose ceil(N*H*W / 64) pixel tiles stay below 2^31
+ * is accepted; earlier versions returned NM_E_UNSUPPORTED for some very large batches. */
 int nm_conv3x3_bias_relu_fwd(const float* x, const float* w, const float* bias,
                              float* y, int64_t N, int64_t H, int64_t W,
                              int64_t Cin, int64_t Cout, void* stream);
@@ -691,7 +693,8 @@ int nm_squared_error_fwd(const float* pred, const float* target, float* loss, in
 int nm_squared_error_bwd(const float* pred, const float* target, const float* dloss, float* dpred, int64_t B,
                          int64_t dim, void* stream);
 
-/* ---- K19: one layer of the convolutional seq2seq encoder (encoders/facebook_conv.py, csrc/glu_conv.cu) ----------
+/* ---- K19: one layer of the convolutional seq2seq encoder (encoders/facebook_conv.py, csrc/glu_conv.cu on the
+ * implicit-GEMM kernels of csrc/conv_igemm.cuh: a 1 x k window over [B, 1, T, F]) ------------------------------
  * x [B,T,F], w [k,F,2F], bias [2F], fp32, row-major; M = B*T.
  *   z = conv1d(x, w) + bias       TF's SAME padding at stride 1: (k-1)/2 zeros before each sequence, the rest after;
  *                                 positions inside [0,T) always take part, padded batch positions included

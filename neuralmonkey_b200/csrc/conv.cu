@@ -2,85 +2,11 @@
 // encoders/imagenet_encoder.py:212,234 of the reference).  NHWC fp32.
 //   conv3x3, stride 1, SAME, + bias + ReLU  (vgg_arg_scope of tensorflow/models slim nets/vgg.py)
 //   max-pool 2x2 / 2
-// The convolution is an implicit GEMM: M = N*H*W output pixels, N = Cout, K = 9*Cin,
-// A(m, (dy,dx,c)) gathered on the fly from the input (zero outside the image), B = the
-// HWIO filter viewed as [9*Cin, Cout].  Round 1 runs the tile on the CUDA cores in exact
-// fp32; a TMA-im2col tensor-core mainloop is listed under "what comes next" in DESIGN.md.
-#include "gemm_simt.cuh"
+// The convolution runs on the exact fp32 CUDA-core kernel of conv_igemm.cuh (k = 3, pads 1, ReLU);
+// nm_im2col3x3 builds the patch matrix for the tensor-core path through nm_gemm.
+#include "conv_igemm.cuh"
 
 namespace nm {
-
-constexpr int CV_BM = 64, CV_BN = 64, CV_TM = 4, CV_TN = 4;
-
-__global__ void __launch_bounds__(SIMT_THREADS)
-conv3x3_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-               float* __restrict__ y, int64_t NB, int H, int W, int Cin, int Cout) {
-  __shared__ SimtSmem<CV_BM, CV_BN, CV_TM, CV_TN> sm;
-  const int64_t M = NB * H * W;
-  const int K = 9 * Cin;
-  const int64_t m0 = (int64_t)blockIdx.y * CV_BM;
-  const int n0 = blockIdx.x * CV_BN;
-  const int t = threadIdx.x;
-  const int tx = t % (CV_BN / CV_TN), ty = t / (CV_BN / CV_TN);
-  float acc[CV_TM][CV_TN];
-#pragma unroll
-  for (int i = 0; i < CV_TM; ++i)
-#pragma unroll
-    for (int j = 0; j < CV_TN; ++j) acc[i][j] = 0.f;
-
-  for (int k0 = 0; k0 < K; k0 += SIMT_BK) {
-    // A tile: element (m, k): k fastest across threads (c is contiguous in NHWC)
-#pragma unroll
-    for (int i = 0; i < (CV_BM * SIMT_BK) / SIMT_THREADS; ++i) {
-      const int idx = t + i * SIMT_THREADS;
-      const int m = idx / SIMT_BK, k = idx % SIMT_BK;
-      const int64_t gm = m0 + m;
-      const int gk = k0 + k;
-      float val = 0.f;
-      if (gm < M && gk < K) {
-        const int tap = gk / Cin, c = gk - tap * Cin;
-        const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-        const int64_t n = gm / ((int64_t)H * W);
-        const int rem = (int)(gm - n * (int64_t)H * W);
-        const int yy = rem / W + dy, xx = rem % W + dx;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W)
-          val = x[((n * H + yy) * W + xx) * Cin + c];
-      }
-      sm.a[k][m] = val;
-    }
-#pragma unroll
-    for (int i = 0; i < (CV_BN * SIMT_BK) / SIMT_THREADS; ++i) {
-      const int idx = t + i * SIMT_THREADS;
-      const int k = idx / CV_BN, n = idx % CV_BN;
-      const int gk = k0 + k, gn = n0 + n;
-      sm.b[k][n] = (gk < K && gn < Cout) ? w[(int64_t)gk * Cout + gn] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < SIMT_BK; ++k) {
-      float av[CV_TM], bv[CV_TN];
-#pragma unroll
-      for (int i = 0; i < CV_TM; ++i) av[i] = sm.a[k][ty * CV_TM + i];
-#pragma unroll
-      for (int j = 0; j < CV_TN; ++j) bv[j] = sm.b[k][tx * CV_TN + j];
-#pragma unroll
-      for (int i = 0; i < CV_TM; ++i)
-#pragma unroll
-        for (int j = 0; j < CV_TN; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < CV_TM; ++i) {
-    const int64_t m = m0 + ty * CV_TM + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < CV_TN; ++j) {
-      const int n = n0 + tx * CV_TN + j;
-      if (n < Cout) y[m * Cout + n] = fmaxf(acc[i][j] + bias[n], 0.f);
-    }
-  }
-}
 
 // im2col for the tensor-core path: cols[m][tap*Cin + c] = x[n, y+dy, x+dx, c] (zero outside the
 // image), row pitch `ldc` floats.  One thread per (pixel, tap, 4-channel group); the group moves as one
@@ -142,39 +68,17 @@ int nm_conv3x3_bias_relu_fwd(const float* x, const float* w, const float* bias, 
   NM_REQUIRE(x && w && bias && y, NM_E_INVALID, "nm_conv3x3_bias_relu_fwd: null pointer");
   NM_REQUIRE(N > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, NM_E_INVALID,
              "nm_conv3x3_bias_relu_fwd: bad sizes");
-  const int64_t M = N * H * W;
-  NM_REQUIRE(ceil_div(M, CV_BM) <= 0x7fffffffLL && ceil_div(Cout, CV_BN) <= 65535, NM_E_UNSUPPORTED,
-             "nm_conv3x3_bias_relu_fwd: grid too large");
-  dim3 grid((unsigned)ceil_div(Cout, CV_BN), (unsigned)ceil_div(M, CV_BM));
-  NM_REQUIRE(grid.y <= 65535u * 16u, NM_E_UNSUPPORTED, "nm_conv3x3_bias_relu_fwd: too many pixels");
-  if (grid.y > 65535u) {
-    // split the batch so grid.y stays within the launch limit
-    const int64_t per = (65535LL * CV_BM) / (H * W);
-    NM_REQUIRE(per >= 1, NM_E_UNSUPPORTED, "nm_conv3x3_bias_relu_fwd: image too large");
-    for (int64_t n0 = 0; n0 < N; n0 += per) {
-      const int64_t nb = (N - n0 < per) ? N - n0 : per;
-      const int rc = nm_conv3x3_bias_relu_fwd(x + n0 * H * W * Cin, w, bias, y + n0 * H * W * Cout, nb,
-                                              H, W, Cin, Cout, stream);
-      if (rc) return rc;
-    }
-    return NM_OK;
-  }
-  conv3x3_kernel<<<grid, SIMT_THREADS, 0, (cudaStream_t)stream>>>(x, w, bias, y, N, (int)H, (int)W,
-                                                                  (int)Cin, (int)Cout);
-  NM_LAUNCH_CHECK("nm_conv3x3_bias_relu_fwd");
-  return NM_OK;
+  const ConvGeom g = conv_geom_of(N, H, W, Cin, Cout, 3, 3, 1, 1, H, W);
+  return conv_fwd_launch<CS_BN, false, false>(x, w, g, BiasAct{bias, y, NM_ACT_RELU}, NM_GEMM_SIMT,
+                                              (cudaStream_t)stream, "nm_conv3x3_bias_relu_fwd");
 }
 
 int nm_im2col3x3(const float* x, float* cols, int64_t N, int64_t H, int64_t W, int64_t Cin,
                  int64_t ldc, void* stream) {
   NM_REQUIRE(x && cols, NM_E_INVALID, "nm_im2col3x3: null pointer");
   NM_REQUIRE(N > 0 && H > 0 && W > 0 && Cin > 0 && ldc >= 9 * Cin, NM_E_INVALID, "nm_im2col3x3: bad sizes");
-  const int64_t total = N * H * W * 9 * ((Cin + 3) / 4);
-  int64_t blocks = ceil_div(total, 256);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  im2col3x3_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, cols, N, (int)H, (int)W, (int)Cin,
-                                                                      ldc);
+  im2col3x3_kernel<<<grid_for(N * H * W * 9 * ((Cin + 3) / 4)), 256, 0, (cudaStream_t)stream>>>(
+      x, cols, N, (int)H, (int)W, (int)Cin, ldc);
   NM_LAUNCH_CHECK("nm_im2col3x3");
   return NM_OK;
 }
@@ -184,11 +88,8 @@ int nm_maxpool2x2_fwd(const float* x, float* y, int64_t N, int64_t H, int64_t W,
   NM_REQUIRE(x && y, NM_E_INVALID, "nm_maxpool2x2_fwd: null pointer");
   NM_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && H % 2 == 0 && W % 2 == 0, NM_E_INVALID,
              "nm_maxpool2x2_fwd: bad sizes (H, W must be even)");
-  const int64_t total = N * (H / 2) * (W / 2) * C;
-  int64_t blocks = ceil_div(total, 256);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  maxpool2x2_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, y, N, (int)H, (int)W, (int)C);
+  maxpool2x2_kernel<<<grid_for(N * (H / 2) * (W / 2) * C), 256, 0, (cudaStream_t)stream>>>(x, y, N, (int)H, (int)W,
+                                                                                           (int)C);
   NM_LAUNCH_CHECK("nm_maxpool2x2_fwd");
   return NM_OK;
 }

@@ -1,7 +1,7 @@
-"""The weight-gradient plans of the convolution kernels (csrc/cnn.cu wgrad_plan, csrc/glu_conv.cu glu_wgrad_plan)
-restated in Python, and named cases that each land on one branch of them.
+"""The weight-gradient plan of the convolution kernels (csrc/conv_igemm.cuh wgrad_plan, for conv2d's and the GLU
+conv's tiles) restated in Python, and named cases that each land on one branch of it.
 
-Both kernels sum dW[r, o] = sum_m A'(r, m) dY(m, o) over the m = output pixels (positions) in k-blocks, split over
+Both convolutions sum dW[r, o] = sum_m A'(r, m) dY(m, o) over the m = output pixels (positions) in k-blocks, split over
 CTAs into a workspace of [rows, cols] slices, rows = (filter taps x input channels) + 1 for the bias row.  The
 split count asks for about 4 CTAs per SM, at most one per k-block, at most what the workspace holds; the k-blocks
 are then dealt out evenly, so the last split may be shorter.  The shapes of a case are not fixed: each case
@@ -39,7 +39,7 @@ def cdiv(a: int, b: int) -> int:
 
 
 def wgrad_plan(rows: int, cols: int, m: int, tiles: Tiles, sms: int, ws_cap: int = -1) -> Plan:
-    """wgrad_plan / glu_wgrad_plan: ws_cap < 0 is an unbounded workspace."""
+    """wgrad_plan: ws_cap < 0 is an unbounded workspace."""
     part = rows * cols
     tiles_r, tiles_o = cdiv(rows, tiles.bm), cdiv(cols, tiles.bn)
     total_kb = cdiv(m, tiles.bk)

@@ -1,5 +1,5 @@
-"""Time the CNN encoder's convolutions (forward, data gradient, weight gradient) at tests/str.ini's own shapes and
-at a CRNN-like stack, next to cuDNN (torch.nn.functional.conv2d with TF32 allowed, alternating with ours in the same
+"""Time the CNN encoder's convolutions (csrc/cnn.cu on the kernels of csrc/conv_igemm.cuh: forward, data gradient,
+weight gradient) at tests/str.ini's own shapes and at a CRNN-like stack, next to cuDNN (torch.nn.functional.conv2d with TF32 allowed, alternating with ours in the same
 process, as a comparison point only), and one full training step of the str.ini model.  Prints a table and one JSON
 line; the card's name and power limit are read in the same run.
 

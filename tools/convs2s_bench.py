@@ -1,5 +1,5 @@
-"""Time one ConvS2S encoder layer (csrc/glu_conv.cu through `ops.conv1d_glu_residual`: conv1d SAME + bias + GLU +
-residual) against the cuDNN composition of the same maths under autograd - `F.conv1d` with TF32 allowed, `F.glu`,
+"""Time one ConvS2S encoder layer (csrc/glu_conv.cu on the kernels of csrc/conv_igemm.cuh, through
+`ops.conv1d_glu_residual`: conv1d SAME + bias + GLU + residual) against the cuDNN composition of the same maths under autograd - `F.conv1d` with TF32 allowed, `F.glu`,
 the add - forward and forward+backward, at the sizes a user runs, and a 6-layer F = 512 encoder stack the same way.
 The two sides alternate in the same process.  TFLOP/s count the convolution's products only (2 * B*T * k*F * 2F per
 forward, three times that per forward+backward); the share of peak is over the 495 TFLOP/s TF32 data-sheet figure of
