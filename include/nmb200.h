@@ -219,6 +219,55 @@ int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask,
                     float* de_work, int64_t B, int64_t Tx, int64_t NQ, int64_t A,
                     int64_t C, void* stream);
 
+/* ---- Coverage attention --------------------------------------------------------
+ * Replaces CoverageAttention (attention/coverage.py:37-61 with
+ * attention/feed_forward.py:125-166) for NQ decoder steps at once, as a scan:
+ *     fert[b,t]  = 1e-8 + max_fertility*sigmoid(sum_c fertility_w[c]*S[b,t,c])
+ *     sum_0      = cov_in (0 when NULL);  sum_{q+1} = sum_q + w[b,q,:]
+ *     cov[b,q,t] = sum_q[t] / fert[b,t] * mask[b,t]
+ *     e[b,q,t]   = sum_a v[a]*tanh(keys[b,t,a] + qproj[b,q,a] + coverage_w[a]*cov[b,q,t])
+ *     w          = softmax_t(e) * mask ;  w /= (sum_t w + 1e-8)   (as K4, no bias)
+ *     ctx[b,q]   = sum_t w[b,q,t] * values[b,t,:];   cov_out = sum_NQ
+ * Fertility: states [B,Tx,C] -> fert [B,Tx], fp32 dot products.  Its backward
+ * overwrites dstates and accumulates into dfertility_w [C]; work is B*C floats. */
+int nm_coverage_fertility_fwd(const float* states, const float* fertility_w,
+                              float max_fertility, float* fert, int64_t B,
+                              int64_t Tx, int64_t C, void* stream);
+int nm_coverage_fertility_bwd(const float* states, const float* fertility_w,
+                              float max_fertility, const float* dfert,
+                              float* dstates, float* dfertility_w, float* work,
+                              int64_t B, int64_t Tx, int64_t C, void* stream);
+/* Attention scan.  keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] (may be NULL),
+ * fert [B,Tx], qproj [B,NQ,A], v [A], coverage_w [A], cov_in [B,Tx] (may be
+ * NULL = zero coverage).  Outputs: energies, weights and coverage [B,NQ,Tx]
+ * (the first and last saved for backward), ctx [B,NQ,C], cov_out [B,Tx].  Each
+ * step's arithmetic is independent of NQ: NQ chained one-step calls give the
+ * bits of one NQ-step call.  Refuses (NM_E_UNSUPPORTED) shapes whose shared
+ * memory, 4*(3A + 4Tx) bytes, exceeds 200 KB. */
+int nm_coverage_attention_fwd(const float* keys, const float* values,
+                              const float* mask, const float* fert,
+                              const float* qproj, const float* v,
+                              const float* coverage_w, const float* cov_in,
+                              float* energies, float* weights, float* coverage,
+                              float* ctx, float* cov_out, int64_t B, int64_t Tx,
+                              int64_t NQ, int64_t A, int64_t C, void* stream);
+/* Reverse scan.  dkeys, dvalues, dqproj, dfert and dcov_in (may be NULL) are
+ * overwritten; dv and dcoverage_w [A] are accumulated into.  dcov_out may be
+ * NULL (zero).  No atomics: repeated calls give identical bits.  work is 2*B*A
+ * floats.  Refuses B > 65535, 4*(51A + C + 6Tx) bytes of shared memory above
+ * 200 KB, or 4*NQ*(Tx rounded up to 8 + 128) bytes above 200 KB. */
+int nm_coverage_attention_bwd(const float* keys, const float* values,
+                              const float* mask, const float* fert,
+                              const float* qproj, const float* v,
+                              const float* coverage_w, const float* energies,
+                              const float* weights, const float* coverage,
+                              const float* dctx, const float* dcov_out,
+                              float* dkeys, float* dvalues, float* dqproj,
+                              float* dfert, float* dcov_in, float* dv,
+                              float* dcoverage_w, float* work, int64_t B,
+                              int64_t Tx, int64_t NQ, int64_t A, int64_t C,
+                              void* stream);
+
 /* ---- Joint multi-source attention --------------------------------------------
  * Replaces FlatMultiAttention.attention (attention/combination.py:240-321) and
  * HierarchicalMultiAttention.attention (:394-463) for NQ query steps at once:

@@ -19,6 +19,7 @@ from neuralmonkey_b200.typecheck import check_argument_types
 from neuralmonkey_b200 import ops
 from neuralmonkey_b200.attention.base_attention import (
     Attendable, BaseAttention, empty_attention_loop_state, get_attention_mask, get_attention_states)
+from neuralmonkey_b200.attention.coverage import CoverageAttention
 from neuralmonkey_b200.attention.namedtuples import AttentionLoopState, HierarchicalLoopState
 from neuralmonkey_b200.decorators import tensor
 from neuralmonkey_b200.model.model_part import ModelPart
@@ -277,6 +278,10 @@ class HierarchicalMultiAttention(MultiAttention):
                                 initializers=initializers)
         if not attentions:
             raise ValueError("HierarchicalMultiAttention '{}' needs at least one attention".format(name))
+        for att in attentions:
+            if isinstance(att, CoverageAttention):
+                raise ValueError("HierarchicalMultiAttention '{}': child '{}' is a CoverageAttention, whose energies "
+                                 "read its loop state; the children are queried without one".format(name, att.name))
         self.attentions = attentions
     # pylint: enable=too-many-arguments
 

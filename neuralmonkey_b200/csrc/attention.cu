@@ -278,6 +278,21 @@ bahdanau_bwd_values_kernel(const float* __restrict__ weights, const float* __res
   }
 }
 
+// The caller has checked att_values_smem(Tx, NQ) against ATT_SMEM_LIMIT and B <= 65535.
+int att_values_grad(const float* weights, const float* dctx, float* dvalues, int64_t B, int64_t Tx, int64_t NQ,
+                    int64_t C, cudaStream_t s) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    NM_CUDA_TRY(cudaFuncSetAttribute(bahdanau_bwd_values_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)ATT_SMEM_LIMIT));
+    attr_set = true;
+  }
+  dim3 grid((unsigned)ceil_div(C, ATT_ACH), (unsigned)B);
+  bahdanau_bwd_values_kernel<<<grid, ATT_ACH, att_values_smem(Tx, NQ), s>>>(weights, dctx, dvalues, (int)Tx,
+                                                                           (int)NQ, (int)C);
+  NM_LAUNCH_CHECK("att_values_grad");
+  return NM_OK;
+}
 
 }  // namespace nm
 

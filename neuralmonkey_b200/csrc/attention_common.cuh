@@ -163,4 +163,12 @@ inline int att_chunks(int64_t B, int64_t NQ) {
   return (int)std::min(NQ, std::max(ceil_div(NQ, ATT_QMAX), want));
 }
 
+// Shared memory of K4's value-gradient kernel, and the kernel itself (attention.cu) for other attentions whose
+// values enter only through ctx = w . values: dvalues[b,t,c] = sum_q weights[b,q,t] dctx[b,q,c].
+inline size_t att_values_smem(int64_t Tx, int64_t NQ) {
+  return sizeof(float) * (size_t)(NQ * ceil_div(Tx, ATT_VT) * ATT_VT + NQ * ATT_ACH);
+}
+int att_values_grad(const float* weights, const float* dctx, float* dvalues, int64_t B, int64_t Tx, int64_t NQ,
+                    int64_t C, cudaStream_t s);
+
 }  // namespace nm

@@ -122,7 +122,11 @@ class BeamSearchDecoder(ModelPart):
         gathered = gathered._replace(
             embedded_input=self.parent_decoder.embed_input_symbols(words.view(-1)),
             finished=finished.view(-1))
-        return self._decoder_step(dec_ls._replace(feedables=gathered))
+        histories = dec_ls.histories
+        reorder = getattr(self.parent_decoder, "reorder_attention_states", None)
+        if reorder is not None:     # loop states the next step's attention energies read (coverage)
+            histories = reorder(histories, lambda x: ops.beam_gather(x, beams, bsz, k))
+        return self._decoder_step(dec_ls._replace(feedables=gathered, histories=histories))
 
     def decoding_loop(self, initial: BeamSearchLoopState) -> BeamSearchOutput:
         k = self.beam_size

@@ -20,6 +20,7 @@ import torch
 from neuralmonkey_b200.typecheck import check_argument_types
 from neuralmonkey_b200 import ops, runtime
 from neuralmonkey_b200.attention.base_attention import BaseAttention
+from neuralmonkey_b200.attention.coverage import CoverageAttention
 from neuralmonkey_b200.decoders.autoregressive import AutoregressiveDecoder, LoopState
 from neuralmonkey_b200.decoders.encoder_projection import (
     EncoderProjection, concat_encoder_projection, empty_initial_state, linear_encoder_projection)
@@ -196,12 +197,16 @@ class Decoder(AutoregressiveDecoder):
             return att.attention_sequence(queries, prev_outputs, inputs)
         return att.attention_sequence(queries)
 
-    def _step_attend(self, prev_output, rnn_input):
+    def _step_attend(self, prev_output, rnn_input, coverage):
         """`attend(att, query)` of one teacher-forced or differentiable step: prev_output is what the step
-        received (the (c, h) pair of an LSTM), rnn_input the step's embedded input."""
+        received (the (c, h) pair of an LSTM), rnn_input the step's embedded input.  `coverage` maps each coverage
+        attention (by id) to its running sum of weights, absent before the first step; `attend` advances it."""
         prev_h = prev_output[1] if isinstance(prev_output, tuple) else prev_output
 
         def attend(att, query):
+            if isinstance(att, CoverageAttention):
+                ctx, w, coverage[id(att)] = att.coverage_scan(query.unsqueeze(1), coverage.get(id(att)))
+                return ctx[:, 0], w
             ctx, w = self._attend_sequence(att, query.unsqueeze(1), prev_h.unsqueeze(1), rnn_input.unsqueeze(1))
             return ctx[:, 0], w
         return attend
@@ -242,9 +247,10 @@ class Decoder(AutoregressiveDecoder):
         prev = self.initial_state
         if self._rnn_cell_str == "LSTM":
             prev = (prev, prev)
-        outputs, cells, weights = [], [], [[] for _ in self.attentions]
+        outputs, cells, weights, coverage = [], [], [[] for _ in self.attentions], {}
         for t in range(fed.shape[1]):       # one query per sentence and step: NQ = 1
-            out, prev, _ctx, attended = self._variant_step(emb[:, t], prev, self._step_attend(prev, emb[:, t]))
+            out, prev, _ctx, attended = self._variant_step(emb[:, t], prev,
+                                                           self._step_attend(prev, emb[:, t], coverage))
             outputs.append(out)
             cells.append(prev[1] if isinstance(prev, tuple) else prev)
             for hist, (_c, w) in zip(weights, attended):
@@ -313,10 +319,10 @@ class Decoder(AutoregressiveDecoder):
         if self._rnn_cell_str == "LSTM":
             prev = (prev, prev)
 
-        states, chosen, argmaxes, masks = [], [], [], []
+        states, chosen, argmaxes, masks, coverage = [], [], [], [], {}
         for step in range(self.max_output_len):
             emb = self.embed_input_symbols(symbols)
-            out, prev, _ctx, _attended = self._variant_step(emb, prev, self._step_attend(prev, emb))
+            out, prev, _ctx, _attended = self._variant_step(emb, prev, self._step_attend(prev, emb, coverage))
             with torch.no_grad():
                 logits, _lse, argmax = self.state_to_logits(out.detach(), keep_logits=sample)
                 if sample:
@@ -367,6 +373,17 @@ class Decoder(AutoregressiveDecoder):
             rnn_outputs=[],
             attention_histories=[a.initial_loop_state() for a in self.attentions if a is not None])
         return histories._replace(other=rnn_histories)
+
+    def reorder_attention_states(self, histories, gather):
+        """`histories` (of this decoder's loop state) with the running coverage of every coverage attention
+        passed through `gather` - the beam search's re-ordering of rows to the selected hypotheses.  The other
+        histories are not read by the next step and stay as they are."""
+        if not any(isinstance(att, CoverageAttention) for att in self.attentions):
+            return histories
+        states = [state._replace(coverage=gather(state.coverage))
+                  if isinstance(att, CoverageAttention) and state.coverage is not None else state
+                  for att, state in zip(self.attentions, histories.other.attention_histories)]
+        return histories._replace(other=histories.other._replace(attention_histories=states))
 
     def next_state(self, loop_state: LoopState) -> Tuple[torch.Tensor, Any, Any]:
         """Decoder.next_state, GRU branch (decoder.py:279-358)."""

@@ -693,6 +693,105 @@ def bahdanau_attention(keys: torch.Tensor, values: torch.Tensor, mask: Optional[
 
 
 # ---------------------------------------------------------------------------
+# Coverage attention (attention.coverage)
+# ---------------------------------------------------------------------------
+class _CoverageFertility(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, states, fertility_w, max_fertility):
+        bsz, tx, c = states.shape
+        states = states.contiguous()
+        fert = torch.empty(bsz, tx, device=states.device, dtype=torch.float32)
+        call("nm_coverage_fertility_fwd", ptr(states), ptr(fertility_w), float(max_fertility), ptr(fert),
+             bsz, tx, c, lib.stream())
+        ctx.save_for_backward(states, fertility_w)
+        ctx.max_fertility = max_fertility
+        ctx.sink = _sink(fertility_w)
+        return fert
+
+    @staticmethod
+    def backward(ctx, dfert):
+        states, fertility_w = ctx.saved_tensors
+        bsz, tx, c = states.shape
+        dev = states.device
+        dfert = dfert.contiguous()
+        dstates = torch.empty_like(states)
+        dfw = ctx.sink if ctx.sink is not None else torch.zeros(c, device=dev, dtype=torch.float32)
+        work = torch.empty(bsz * c, device=dev, dtype=torch.float32)
+        call("nm_coverage_fertility_bwd", ptr(states), ptr(fertility_w), ctx.max_fertility,
+             ptr(dfert), ptr(dstates), ptr(dfw), ptr(work), bsz, tx, c, lib.stream())
+        return dstates, None if ctx.sink is not None else dfw, None
+
+
+def coverage_fertility(states: torch.Tensor, fertility_w: torch.Tensor, max_fertility: float) -> torch.Tensor:
+    """CoverageAttention.fertility (attention/coverage.py:47-50): 1e-8 + max_fertility * sigmoid(states .
+    fertility_w) in fp32 dot products.  states [B,Tx,C], fertility_w [C] -> fert [B,Tx]."""
+    return _CoverageFertility.apply(states, fertility_w, float(max_fertility))
+
+
+class _CoverageAttention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keys, values, mask, fert, qproj, v, coverage_w, cov_in):
+        bsz, tx, a = keys.shape
+        c = values.size(2)
+        nq = qproj.size(1)
+        keys, values, fert, qproj = keys.contiguous(), values.contiguous(), fert.contiguous(), qproj.contiguous()
+        mask_c = mask.contiguous() if mask is not None else None
+        cov_in_c = cov_in.contiguous() if cov_in is not None else None
+        dev = keys.device
+        energies = torch.empty(bsz, nq, tx, device=dev, dtype=torch.float32)
+        weights = torch.empty(bsz, nq, tx, device=dev, dtype=torch.float32)
+        coverage = torch.empty(bsz, nq, tx, device=dev, dtype=torch.float32)
+        ctxv = torch.empty(bsz, nq, c, device=dev, dtype=torch.float32)
+        cov_out = torch.empty(bsz, tx, device=dev, dtype=torch.float32)
+        call("nm_coverage_attention_fwd", ptr(keys), ptr(values), ptr(mask_c), ptr(fert), ptr(qproj), ptr(v),
+             ptr(coverage_w), ptr(cov_in_c), ptr(energies), ptr(weights), ptr(coverage), ptr(ctxv), ptr(cov_out),
+             bsz, tx, nq, a, c, lib.stream())
+        ctx.save_for_backward(keys, values, mask_c, fert, qproj, v, coverage_w, energies, weights, coverage)
+        ctx.sinks = (_sink(v), _sink(coverage_w))
+        ctx.has_cov_in = cov_in is not None
+        ctx.mark_non_differentiable(weights)
+        return ctxv, weights, cov_out
+
+    @staticmethod
+    def backward(ctx, dctx, _dweights, dcov_out):
+        keys, values, mask, fert, qproj, v, coverage_w, energies, weights, coverage = ctx.saved_tensors
+        bsz, tx, a = keys.shape
+        c = values.size(2)
+        nq = qproj.size(1)
+        dev = keys.device
+        dctx = dctx.contiguous()
+        dcov_out = dcov_out.contiguous() if dcov_out is not None else None
+        dkeys = torch.empty_like(keys)
+        dvalues = torch.empty_like(values)
+        dq = torch.empty_like(qproj)
+        dfert = torch.empty_like(fert)
+        dcov_in = torch.empty(bsz, tx, device=dev, dtype=torch.float32) if ctx.has_cov_in else None
+        sv, sc = ctx.sinks
+        dv = sv if sv is not None else torch.zeros(a, device=dev, dtype=torch.float32)
+        dcw = sc if sc is not None else torch.zeros(a, device=dev, dtype=torch.float32)
+        work = torch.empty(2 * bsz * a, device=dev, dtype=torch.float32)
+        call("nm_coverage_attention_bwd", ptr(keys), ptr(values), ptr(mask), ptr(fert), ptr(qproj), ptr(v),
+             ptr(coverage_w), ptr(energies), ptr(weights), ptr(coverage), ptr(dctx), ptr(dcov_out), ptr(dkeys),
+             ptr(dvalues), ptr(dq), ptr(dfert), ptr(dcov_in), ptr(dv), ptr(dcw), ptr(work), bsz, tx, nq, a, c,
+             lib.stream())
+        return (dkeys, dvalues, None, dfert, dq, None if sv is not None else dv, None if sc is not None else dcw,
+                dcov_in)
+
+
+def coverage_attention(keys: torch.Tensor, values: torch.Tensor, mask: Optional[torch.Tensor], fert: torch.Tensor,
+                       qproj: torch.Tensor, v: torch.Tensor, coverage_w: torch.Tensor,
+                       cov_in: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """CoverageAttention.attention (attention/coverage.py:52-61 in feed_forward.py:125-166) for NQ consecutive
+    decoder steps, as one scan.
+
+    keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] or None, fert [B,Tx] (`coverage_fertility`), qproj [B,NQ,A],
+    v [A], coverage_w [A], cov_in [B,Tx]: the sum of the weights of earlier steps, None for none.  Returns
+    (contexts [B,NQ,C], weights [B,NQ,Tx], cov_out [B,Tx] = cov_in + the sum of the NQ steps' weights).  The
+    weights are not differentiable; the gradient between calls flows through cov_out."""
+    return _CoverageAttention.apply(keys, values, mask, fert, qproj, v, coverage_w, cov_in)
+
+
+# ---------------------------------------------------------------------------
 # Joint multi-source attention (attention.combination)
 # ---------------------------------------------------------------------------
 class _JointAttention(torch.autograd.Function):
