@@ -601,7 +601,8 @@ int nm_lstm_gate_bwd(const float* dnew_c, const float* dnew_h, const float* save
  *   Wo [H+E+C, O] (or [H+E+C, 2*O] with maxout != 0), bo; act = NM_ACT_* (ignored with maxout).
  * Outputs: h_out [rows,H]; out [rows,O]; optional x_out [rows,E] (embedded input), ctx_out [rows,C],
  * weights_out [rows,Tx].  16-byte loads and TMA-staged key/value tiles need E,H,A,C,O % 4 == 0 and
- * 16-byte aligned bases; other shapes take a scalar variant of the same kernel. */
+ * 16-byte aligned bases; other shapes take a scalar variant of the same kernel.  Shapes the kernel cannot
+ * take (nm_attn_decoder_step_supported returns 0) return NM_E_UNSUPPORTED before anything is launched. */
 int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, const float* x_in,
                              const float* h_prev, const int32_t* parent, const float* Wg, const float* bg,
                              const float* Wc, const float* bc, const float* Wq, const float* bq,
@@ -610,6 +611,13 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
                              float* x_out, float* h_out, float* ctx_out, float* weights_out, float* out,
                              int64_t rows, int64_t group, int64_t E, int64_t H, int64_t A, int64_t C,
                              int64_t Tx, int64_t O, int act, int maxout, void* stream);
+
+/* 1 when nm_attn_decoder_step_fwd takes this shape on the current device (its SM count picks the cluster
+ * size, which sizes the shared memory), else 0: the context (C <= 512, or C <= 2048 on the vector variant),
+ * one key / value tile and the step's shared memory must fit one CTA.  `aligned` != 0: Wg, Wc, Wq, Wo, keys
+ * and values are 16-byte aligned. */
+int nm_attn_decoder_step_supported(int64_t rows, int64_t group, int64_t E, int64_t H, int64_t A, int64_t C,
+                                   int64_t Tx, int64_t O, int maxout, int aligned);
 
 /* Diagnostic: 8 int64 device counters receiving the cycle counter of CTA 0 at the phase boundaries of the
  * following nm_attn_decoder_step_fwd launches; NULL switches it off. */

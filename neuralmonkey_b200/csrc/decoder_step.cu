@@ -155,6 +155,7 @@ __device__ __noinline__ void ds_panel(const DsSeg* segs, int nseg, int K, const 
                                       int ldw, int colA, int nA, int colB, int nB,
                                       float* __restrict__ res, int res_ld, float* __restrict__ red) {
   const int ng = nA + nB;
+  if (ng == 0) return;   // a CTA of a large cluster may own no columns of a small product (uniform per CTA)
   constexpr int RG = DS_R * G;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // groups per warp: the choice that keeps most warps busy (38 groups: gw = 8 -> 5 quads x 3 warps; gw = 4
@@ -646,6 +647,63 @@ using namespace nm;
 
 static long long* g_decstep_prof = nullptr;
 
+// 227 KB per CTA minus the kernel's static shared memory (the run table), rounded up to 1 KB
+constexpr int DS_MAX_DYN_SMEM = 227 * 1024 - 1024;
+
+// The launch plan of one step: sizes, cluster size, vector or scalar variant, ring slot and tile lengths, and
+// the dynamic shared memory, from the sizes, the SM count of the current device and whether every base the
+// vector variant reads with 16-byte loads is 16-byte aligned.  NM_E_UNSUPPORTED (message set) for the shapes
+// the kernel cannot take: nm_attn_decoder_step_supported and the launcher answer from this one function.
+static int ds_plan(int64_t rows, int64_t group, int64_t E, int64_t H, int64_t A, int64_t C, int64_t Tx, int64_t O,
+                   int maxout, bool aligned, DecStep& p, bool& vec, size_t& smem_bytes) {
+  NM_REQUIRE(rows > 0 && group > 0 && E > 0 && H > 0 && A > 0 && C > 0 && Tx > 0 && O > 0, NM_E_INVALID,
+             "nm_attn_decoder_step_fwd: bad sizes");
+  NM_REQUIRE(rows < (1 << 24) && Tx < (1 << 20), NM_E_UNSUPPORTED, "nm_attn_decoder_step_fwd: too large");
+  p.rows = (int)rows; p.E = (int)E; p.H = (int)H; p.A = (int)A; p.C = (int)C; p.Tx = (int)Tx; p.O = (int)O;
+  p.group = (int)group; p.maxout = maxout ? 1 : 0;
+
+  vec = (E % 4 == 0) && (H % 4 == 0) && (A % 4 == 0) && (C % 4 == 0) && (O % 4 == 0) && aligned;
+  const int g = vec ? 4 : 1;
+  NM_REQUIRE(ceil_div(C, g) <= DS_THREADS, NM_E_UNSUPPORTED,
+             "nm_attn_decoder_step_fwd: context size %lld too large for one CTA", (long long)C);
+
+  // cluster size: as many CTAs as fill the chip, at most 8, at least one attended row per CTA
+  const int64_t clusters = ceil_div(rows, DS_R);
+  int cl = 8;
+  while (cl > 1 && clusters * cl > (int64_t)sm_count()) cl >>= 1;
+  const char* env = getenv("NMB200_DECSTEP_CLUSTER");
+  if (env && *env) {
+    const int want = atoi(env);
+    if (want == 1 || want == 2 || want == 4 || want == 8) cl = want;
+  }
+  p.cl = cl;
+
+  // ring slots: as large as the shared memory left over allows, whole time steps of keys / values
+  if (vec) {
+    p.slot_floats = 0;
+    const DsLayout base = ds_layout(p, true);
+    const int64_t avail = (int64_t)DS_MAX_DYN_SMEM / 4 - base.total;
+    int64_t slot = avail / DS_SLOTS;
+    slot -= slot % 32;                                       // 128-byte granularity
+    const int64_t need = (A > C ? A : C);
+    NM_REQUIRE(slot >= need, NM_E_UNSUPPORTED,
+               "nm_attn_decoder_step_fwd: sizes leave no room for a key/value tile in shared memory");
+    int64_t cap = 8192;                                      // 32 KB per tile is plenty
+    if (slot > cap) slot = cap - cap % 32;
+    if (slot < need) slot = (need + 31) / 32 * 32;
+    p.slot_floats = (int)slot;
+    p.tck = (int)(slot / A); if (p.tck > Tx) p.tck = (int)Tx;
+    p.tcv = (int)(slot / C); if (p.tcv > Tx) p.tcv = (int)Tx;
+    smem_bytes = sizeof(float) * (size_t)ds_layout(p, true).total;
+  } else {
+    p.slot_floats = 0; p.tck = (int)Tx; p.tcv = (int)Tx;
+    smem_bytes = sizeof(float) * (size_t)ds_layout(p, false).total;
+  }
+  NM_REQUIRE(smem_bytes <= (size_t)DS_MAX_DYN_SMEM, NM_E_UNSUPPORTED,
+             "nm_attn_decoder_step_fwd: needs %zu bytes of shared memory", smem_bytes);
+  return NM_OK;
+}
+
 extern "C" {
 
 /* Diagnostic: 8 int64 device counters receiving clock64() of CTA 0 at the phase boundaries of the next
@@ -670,63 +728,20 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
                  h_out && out,
              NM_E_INVALID, "nm_attn_decoder_step_fwd: null pointer");
   NM_REQUIRE(h_prev != h_out, NM_E_INVALID, "nm_attn_decoder_step_fwd: h_out must not alias h_prev");
-  NM_REQUIRE(rows > 0 && group > 0 && E > 0 && H > 0 && A > 0 && C > 0 && Tx > 0 && O > 0, NM_E_INVALID,
-             "nm_attn_decoder_step_fwd: bad sizes");
-  NM_REQUIRE(rows < (1 << 24) && Tx < (1 << 20), NM_E_UNSUPPORTED, "nm_attn_decoder_step_fwd: too large");
+  // vector path: every row the kernel reads with 16-byte loads is 16-byte aligned
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool aligned = al16(Wg) && al16(Wc) && al16(Wq) && al16(Wo) && al16(keys) && al16(values);
   DecStep p{};
-  p.rows = (int)rows; p.E = (int)E; p.H = (int)H; p.A = (int)A; p.C = (int)C; p.Tx = (int)Tx; p.O = (int)O;
-  p.group = (int)group; p.act = act; p.maxout = maxout ? 1 : 0;
+  bool vec = false;
+  size_t smem_bytes = 0;
+  const int rc = ds_plan(rows, group, E, H, A, C, Tx, O, maxout, aligned, p, vec, smem_bytes);
+  if (rc != NM_OK) return rc;
+  p.act = act;
   p.symbols = x_in ? nullptr : symbols; p.table = emb_table; p.x_in = x_in; p.h_prev = h_prev; p.parent = parent;
   p.Wg = Wg; p.bg = bg; p.Wc = Wc; p.bc = bc; p.Wq = Wq; p.bq = bq; p.v = v; p.abias = att_bias;
   p.keys = keys; p.values = values; p.mask = mask; p.Wo = Wo; p.bo = bo;
   p.x_out = x_out; p.h_out = h_out; p.ctx_out = ctx_out; p.w_out = weights_out; p.out = out;
   p.prof = g_decstep_prof;
-
-  // vector path: every row the kernel reads with 16-byte loads is 16-byte aligned
-  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  const bool vec = (E % 4 == 0) && (H % 4 == 0) && (A % 4 == 0) && (C % 4 == 0) && (O % 4 == 0) &&
-                   al16(Wg) && al16(Wc) && al16(Wq) && al16(Wo) && al16(keys) && al16(values);
-  const int g = vec ? 4 : 1;
-  NM_REQUIRE(ceil_div(C, g) <= DS_THREADS, NM_E_UNSUPPORTED,
-             "nm_attn_decoder_step_fwd: context size %lld too large for one CTA", (long long)C);
-
-  // cluster size: as many CTAs as fill the chip, at most 8, at least one attended row per CTA
-  const int64_t clusters = ceil_div(rows, DS_R);
-  int cl = 8;
-  while (cl > 1 && clusters * cl > (int64_t)sm_count()) cl >>= 1;
-  const char* env = getenv("NMB200_DECSTEP_CLUSTER");
-  if (env && *env) {
-    const int want = atoi(env);
-    if (want == 1 || want == 2 || want == 4 || want == 8) cl = want;
-  }
-  p.cl = cl;
-
-  // ring slots: as large as the shared memory left over allows, whole time steps of keys / values
-  size_t smem_bytes = 0;
-  if (vec) {
-    p.slot_floats = 0;
-    const DsLayout base = ds_layout(p, true);
-    const int64_t avail = (int64_t)(227 * 1024 - 1024) / 4 - base.total;
-    int64_t slot = avail / DS_SLOTS;
-    slot -= slot % 32;                                       // 128-byte granularity
-    const int64_t need = (A > C ? A : C);
-    NM_REQUIRE(slot >= need, NM_E_UNSUPPORTED,
-               "nm_attn_decoder_step_fwd: sizes leave no room for a key/value tile in shared memory");
-    int64_t cap = 8192;                                      // 32 KB per tile is plenty
-    if (slot > cap) slot = cap - cap % 32;
-    if (slot < need) slot = (need + 31) / 32 * 32;
-    p.slot_floats = (int)slot;
-    p.tck = (int)(slot / A); if (p.tck > Tx) p.tck = (int)Tx;
-    p.tcv = (int)(slot / C); if (p.tcv > Tx) p.tcv = (int)Tx;
-    smem_bytes = sizeof(float) * (size_t)ds_layout(p, true).total;
-  } else {
-    p.slot_floats = 0; p.tck = (int)Tx; p.tcv = (int)Tx;
-    smem_bytes = sizeof(float) * (size_t)ds_layout(p, false).total;
-  }
-  // 227 KB per CTA minus the kernel's static shared memory (the run table), rounded up to 1 KB
-  constexpr int DS_MAX_DYN_SMEM = 227 * 1024 - 1024;
-  NM_REQUIRE(smem_bytes <= (size_t)DS_MAX_DYN_SMEM, NM_E_UNSUPPORTED,
-             "nm_attn_decoder_step_fwd: needs %zu bytes of shared memory", smem_bytes);
 
   auto kern = vec ? attn_decoder_step_kernel<4> : attn_decoder_step_kernel<1>;
   static bool attr_done[2] = {false, false};
@@ -735,13 +750,13 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
     attr_done[vec] = true;
   }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(clusters * cl));
+  cfg.gridDim = dim3((unsigned)(ceil_div(rows, DS_R) * p.cl));
   cfg.blockDim = dim3(DS_THREADS);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = (cudaStream_t)stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)cl;
+  attr[0].val.clusterDim.x = (unsigned)p.cl;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
@@ -749,6 +764,14 @@ int nm_attn_decoder_step_fwd(const int64_t* symbols, const float* emb_table, con
   NM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, p));
   NM_LAUNCH_CHECK("nm_attn_decoder_step_fwd");
   return NM_OK;
+}
+
+int nm_attn_decoder_step_supported(int64_t rows, int64_t group, int64_t E, int64_t H, int64_t A, int64_t C,
+                                   int64_t Tx, int64_t O, int maxout, int aligned) {
+  DecStep p{};
+  bool vec = false;
+  size_t smem_bytes = 0;
+  return ds_plan(rows, group, E, H, A, C, Tx, O, maxout, aligned != 0, p, vec, smem_bytes) == NM_OK;
 }
 
 }  // extern "C"

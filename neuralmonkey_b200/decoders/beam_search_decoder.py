@@ -257,7 +257,7 @@ class BeamSearchDecoder(ModelPart):
     def outputs(self) -> BeamSearchOutput:
         parent = self.parent_decoder
         engine = getattr(parent, "decode_engine", None) if self.use_fused_step else None
-        if engine is not None:
+        if engine is not None and engine.fits(parent.batch_size * self.beam_size, self.beam_size):
             # RNN parent: the fused step kernel follows the beam indices itself and reads the UN-tiled
             # encoder tensors (`group` = beam size), so nothing is tiled or re-gathered here
             return self._fused_outputs(engine)

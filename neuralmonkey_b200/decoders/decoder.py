@@ -443,7 +443,8 @@ class Decoder(AutoregressiveDecoder):
     @tensor
     def _runtime(self):
         engine = self.decode_engine
-        if engine is None or (self.train_mode and self.dropout_keep_prob < 1.0):
+        if (engine is None or (self.train_mode and self.dropout_keep_prob < 1.0)
+                or not engine.fits(self.batch_size, 1)):
             return AutoregressiveDecoder._runtime.fget(self)
         gold = gold_mask = None
         if self._train_ids_host is not None:

@@ -91,6 +91,17 @@ class RNNDecodeEngine:
         return dict(E=dec.embedding_size, H=dec.rnn_size, A=att.state_size, C=att.context_vector_size,
                     O=dec.output_dimension, V=len(dec.vocabulary))
 
+    def fits(self, rows: int, group: int) -> bool:
+        """Whether the step kernel takes `rows` hypotheses (`group` per sentence) over the current encoder states
+        on this device.  It refuses a context wider than one CTA covers, or a step whose shared memory (which
+        grows with the encoder length) does not fit; the decoder then decodes that batch step by step."""
+        d, w = self._dims(), self._weights()
+        tx = self.att.hidden_features.shape[1]
+        # keys and values are copied into buffers of this engine: fresh allocations, 16-byte aligned
+        aligned = all(w[k].data_ptr() % 16 == 0 for k in ("wg", "wc", "wq", "wo"))
+        return bool(lib.load().nm_attn_decoder_step_supported(rows, group, d["E"], d["H"], d["A"], d["C"], tx,
+                                                              d["O"], w["maxout"], int(aligned)))
+
     # -- static buffers ------------------------------------------------------------------------------
     def _buffers(self, key, rows: int, nb: int, tx: int, steps: int, beam: int) -> Dict[str, torch.Tensor]:
         if key in self.bufs:

@@ -19,13 +19,14 @@ MID = dict(vs=120, vt=200, es=32, he=16, et=32, hd=32, out=32, maxout=False, max
 ACT_FN = {"none": lambda z: z, "tanh": torch.tanh, "relu": torch.relu, "sigmoid": torch.sigmoid}
 
 
-def _step_reference(p, symbols, h_prev, parent, group, act="tanh"):
-    """fp64 restatement of one step for rows [rows]; p: dict of fp32 CPU tensors.  `act` is the activation of
-    a dense output projection (ignored with maxout)."""
+def _step_reference(p, symbols, h_prev, parent, group, act="tanh", chunk=64):
+    """fp64 restatement of one step for rows [rows]; p: dict of fp32 tensors, on the CPU or the device (computed
+    there, the attention `chunk` rows at a time).  `act` is the activation of a dense output projection (ignored
+    with maxout)."""
     d = {k: (v.double() if torch.is_tensor(v) and v.dtype == torch.float32 else v) for k, v in p.items()}
-    rows = symbols.shape[0]
+    rows, dev = symbols.shape[0], d["keys"].device
     x = d["table"][symbols]
-    src = torch.arange(rows)
+    src = torch.arange(rows, device=dev)
     if parent is not None:
         src = (src // group) * group + parent.long()
     h = h_prev.double()[src]
@@ -35,14 +36,17 @@ def _step_reference(p, symbols, h_prev, parent, group, act="tanh"):
     c = torch.tanh(torch.cat([x, r * h], 1) @ d["wc"] + d["bc"])
     hn = u * h + (1 - u) * c
     q = hn @ d["wq"] + d["bq"]
-    enc = torch.arange(rows) // group
-    keys, values = d["keys"][enc], d["values"][enc]
-    e = (torch.tanh(keys + q[:, None, :]) * d["v"]).sum(-1) + d["ab"]
-    w = torch.softmax(e, -1)
-    if d["mask"] is not None:
-        w = w * d["mask"][enc]
-        w = w / (w.sum(-1, keepdim=True) + 1e-8)
-    ctx = (w[:, :, None] * values).sum(1)
+    ws, ctxs = [], []
+    for s in range(0, rows, chunk):
+        enc = torch.arange(s, min(rows, s + chunk), device=dev) // group
+        e = (torch.tanh(d["keys"][enc] + q[s:s + chunk, None, :]) * d["v"]).sum(-1) + d["ab"]
+        w = torch.softmax(e, -1)
+        if d["mask"] is not None:
+            w = w * d["mask"][enc]
+            w = w / (w.sum(-1, keepdim=True) + 1e-8)
+        ws.append(w)
+        ctxs.append(torch.bmm(w[:, None, :], d["values"][enc])[:, 0])
+    w, ctx = torch.cat(ws), torch.cat(ctxs)
     z = torch.cat([hn, x, ctx], 1) @ d["wo"] + d["bo"]
     if p["maxout"]:
         o = z.shape[1] // 2
@@ -52,40 +56,41 @@ def _step_reference(p, symbols, h_prev, parent, group, act="tanh"):
     return hn, ctx, w, out
 
 
-def _step_inputs(dims):
-    """Random parameters, symbols, previous states and parents of one step (fp32 CPU tensors)."""
+def _step_inputs(dims, device="cpu"):
+    """Random parameters, symbols, previous states and parents of one step (fp32 tensors on `device`)."""
     rows, group, e, h, a, c, tx, o, maxout, masked = dims[:10]
-    g = torch.Generator().manual_seed(rows * 7 + tx)
+    g = torch.Generator(device).manual_seed(rows * 7 + tx)
     vocab, nb = 50, rows // group
 
     def rnd(*shape, scale=0.3):
-        return torch.randn(*shape, generator=g) * scale
+        return torch.randn(*shape, generator=g, device=device) * scale
 
     p = dict(table=rnd(vocab, e), wg=rnd(e + h, 2 * h), bg=rnd(2 * h) + 1.0, wc=rnd(e + h, h), bc=rnd(h),
              wq=rnd(h, a), bq=rnd(a), v=rnd(a), ab=rnd(1), keys=rnd(nb, tx, a, scale=0.7),
              values=rnd(nb, tx, c, scale=0.7), wo=rnd(h + e + c, (2 if maxout else 1) * o), bo=rnd((2 if maxout else 1) * o),
              maxout=maxout, mask=None)
     if masked:
-        lens = torch.randint(1, tx + 1, (nb,), generator=g)
+        lens = torch.randint(1, tx + 1, (nb,), generator=g, device=device)
         lens[0] = tx
-        p["mask"] = (torch.arange(tx)[None, :] < lens[:, None]).float()
-    symbols = torch.randint(0, vocab, (rows,), generator=g)
+        p["mask"] = (torch.arange(tx, device=device)[None, :] < lens[:, None]).float()
+    symbols = torch.randint(0, vocab, (rows,), generator=g, device=device)
     h_prev = rnd(rows, h, scale=0.5)
-    parent = torch.randint(0, group, (rows,), generator=g).int() if group > 1 else None
+    parent = torch.randint(0, group, (rows,), generator=g, device=device).int() if group > 1 else None
     return p, symbols, h_prev, parent
 
 
-def _run_step(dims, p, symbols, h_prev, parent, act="tanh", x_in=None, outputs=("x", "ctx", "w")):
+def _run_step(dims, p, symbols, h_prev, parent, act="tanh", x_in=None, outputs=("x", "ctx", "w"), spare=0,
+              res=None):
     """One nm_attn_decoder_step_fwd launch; symbols go through the table unless x_in [rows, E] is given.  The
-    optional outputs not named in `outputs` are passed as NULL.  Returns {name: CUDA tensor}."""
+    optional outputs not named in `outputs` are passed as NULL.  Returns {name: CUDA tensor} of NaN-filled outputs
+    with `spare` rows past `rows` (or writes into `res`)."""
     from neuralmonkey_b200 import lib
     rows, group, e, h, a, c, tx, o, maxout, masked = dims[:10]
     dv = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in p.items()}
-    res = {"h": torch.full((rows, h), float("nan"), device="cuda"),
-           "out": torch.full((rows, o), float("nan"), device="cuda")}
-    for name, width in (("x", e), ("ctx", c), ("w", tx)):
-        if name in outputs:
-            res[name] = torch.full((rows, width), float("nan"), device="cuda")
+    if res is None:
+        res = {name: torch.full((rows + spare, width), float("nan"), device="cuda")
+               for name, width in (("h", h), ("out", o), ("x", e), ("ctx", c), ("w", tx))
+               if name in ("h", "out") + tuple(outputs)}
     # held in variables until the launch has run: the kernel only gets their raw pointers
     sym_d, hp_d = symbols.cuda(), h_prev.cuda()
     x_d = x_in.cuda() if x_in is not None else None
