@@ -513,6 +513,27 @@ int nm_im2col3x3(const float* x, float* cols, int64_t N, int64_t H, int64_t W,
 int nm_maxpool2x2_fwd(const float* x, float* y, int64_t N, int64_t H, int64_t W,
                       int64_t C, void* stream);
 
+/* ---- K12: ResNet-v2 convolutions (forward only; the encoder is frozen, encoders/imagenet_encoder.py:70-99
+ * builds slim nets/resnet_v2.py) ---------------------------------------------------------------------------------
+ * y [N,Ho,Wo,Cout] = act(z + r), NHWC fp32, w [k,k,Cin,Cout] (HWIO), with
+ *   A = relu(x * in_scale[c] + in_shift[c]) inside the image and 0 in the padding when in_scale is non-NULL, else x
+ *       (the preactivation batch norm of a v2 unit, never written to memory);
+ *   acc[n,oy,ox,o] = sum over the k x k window at (oy*stride - pad_top, ox*stride - pad_left) of A * w;
+ *   z = acc * out_scale[o] + out_shift[o] when out_scale is non-NULL (an inference-mode batch norm), else acc + bias[o]
+ *       (bias may be NULL; out_scale and bias exclude each other);
+ *   r = res[n, oy*res_stride, ox*res_stride, o] when res is non-NULL (res [N,res_H,res_W,Cout], res_stride 1 or 2,
+ *       ceil(res_H / res_stride) = Ho, ceil(res_W / res_stride) = Wo: the identity shortcut, subsampled in a strided
+ *       unit), else 0.
+ * Ho = (H + pad_top + pad_bottom - k) / stride + 1 (Wo likewise); pads lie in [0, k).  The scale / shift pairs come
+ * together.  act is NM_ACT_NONE or NM_ACT_RELU.  backend: NM_GEMM_SIMT = exact fp32 on the CUDA cores, NM_GEMM_AUTO /
+ * NM_GEMM_TC = wgmma with TF32 operands (the implicit-GEMM kernels of csrc/conv_igemm.cuh).  Bad arguments return
+ * NM_E_INVALID or NM_E_UNSUPPORTED with a message and launch nothing. */
+int nm_conv2d_bn_fwd(const float* x, const float* w, const float* in_scale, const float* in_shift,
+                     const float* out_scale, const float* out_shift, const float* bias, const float* res,
+                     int64_t res_H, int64_t res_W, int64_t res_stride, float* y, int64_t N, int64_t H, int64_t W,
+                     int64_t Cin, int64_t Cout, int64_t k, int64_t stride, int64_t pad_top, int64_t pad_bottom,
+                     int64_t pad_left, int64_t pad_right, int act, int backend, void* stream);
+
 /* ---- K12b: trainable CNN layers (encoders/cnn_encoder.py:209-320: tf.layers.conv2d, batch_normalization,
  * max_pooling2d / average_pooling2d) --------------------------------------------------------------------------
  * NHWC fp32, filters HWIO.  Convolutions have stride 1 (the reference never strides them).

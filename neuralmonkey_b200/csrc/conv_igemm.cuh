@@ -9,6 +9,10 @@
 // product dW[(tap, c), o] = sum_m A(m, (tap, c)) dY(m, o), split over CTAs along m into a caller-owned workspace and
 // summed in a fixed order; one extra row of ones in A gives the bias gradient in the same pass.
 //
+// The forward kernels also take an input policy: the ResNet-v2 convolutions (conv.cu) read x at a stride s,
+// A(m, (tap, c)) = pre(x[n, oy*s + ky - pt, ox*s + kx - pl, c]) with an optional batch norm + ReLU `pre`; every other
+// caller takes the stride-1 default.
+//
 // The GLU conv1d is the one-row case (ONE_ROW: H = kh = 1, pt = 0, W = T): row m of A is then one contiguous span
 // of x cut at the row ends, so its gathers decode the window position only once.
 //
@@ -100,6 +104,31 @@ __device__ __forceinline__ float conv_a(const float* __restrict__ x, const ConvG
 __device__ __forceinline__ float act_apply(float v, int act) { return act == NM_ACT_RELU ? fmaxf(v, 0.f) : v; }
 
 // ------------------------------------------------------------------------------------------------------------
+// Input policies of the forward kernels: how a window reads x.  A stride s places output pixel (oy, ox)'s window at
+// (oy*s - pt, ox*s - pl), so the decoded pixel carries oy*s, ox*s and conv_a_at stays the stride-1 code.
+// ------------------------------------------------------------------------------------------------------------
+// stride 1, A = x: every convolution but the ResNet-v2 ones (the template default)
+struct PlainIn {
+  static constexpr bool ON = false;
+};
+
+// stride s, and when scale is non-NULL A = relu(x * scale[c] + shift[c]) inside the image (0 in the padding): the
+// batch-norm preactivation of a ResNet-v2 unit fused into the gathers of the convolutions that read it
+struct BnReluIn {
+  const float* __restrict__ scale;   // may be NULL
+  const float* __restrict__ shift;
+  int s;
+  static constexpr bool ON = true;
+  __device__ __forceinline__ void origin(Pix& p) const {
+    p.oy *= s;
+    p.ox *= s;
+  }
+  __device__ __forceinline__ float apply(float v, int c) const {
+    return scale ? fmaxf(fmaf(v, __ldg(scale + c), __ldg(shift + c)), 0.f) : v;
+  }
+};
+
+// ------------------------------------------------------------------------------------------------------------
 // Output policies of the forward kernels.  cols() is the width of the output the grid's y axis tiles.  A GATED
 // tile multiplies output column f and its gate column cols + f together and stores both through one call.
 // ------------------------------------------------------------------------------------------------------------
@@ -145,6 +174,30 @@ struct Glu {
   }
 };
 
+// y[m, o] = act(z + res[n, oy*rs, ox*rs, o]) with z = acc * scale[o] + shift[o] (an inference-mode batch norm) when
+// scale is non-NULL, else acc + bias[o]; res [N, Hr, Wr, K] may be NULL.  The ResNet-v2 convolutions.
+struct BnRes {
+  const float* __restrict__ scale;   // may be NULL
+  const float* __restrict__ shift;
+  const float* __restrict__ bias;    // may be NULL
+  const float* __restrict__ res;     // may be NULL
+  float* __restrict__ y;
+  int act, rs, Hr, Wr;
+  static constexpr bool GATED = false;
+  __host__ __device__ int cols(const ConvGeom& g) const { return g.K; }
+  __device__ __forceinline__ void operator()(const ConvGeom& g, int64_t m, int o, float v) const {
+    float z = scale ? fmaf(v, __ldg(scale + o), __ldg(shift + o)) : v + (bias ? __ldg(bias + o) : 0.f);
+    if (res) {
+      const int64_t hw = (int64_t)g.Ho * g.Wo;
+      const int64_t n = m / hw;
+      const int r = (int)(m - n * hw);
+      const int oy = r / g.Wo, ox = r - oy * g.Wo;
+      z += __ldg(res + ((n * Hr + (int64_t)oy * rs) * Wr + (int64_t)ox * rs) * g.K + o);
+    }
+    y[m * g.K + o] = act_apply(z, act);
+  }
+};
+
 // ------------------------------------------------------------------------------------------------------------
 // wgmma engine: 128 x BN output tile, 2 consumer warpgroups of 64 rows, 32-wide k-blocks in a 2-stage ring.
 // All 256 threads gather the next k-block while the tensor cores work on the current one.  A gated tile holds the
@@ -170,10 +223,11 @@ __device__ __forceinline__ void ct_mma(float (&acc)[BN / 2], uint32_t stage_addr
   wgmma_commit();
 }
 
-// Forward / data gradient: epi(m, o, sum A(m, :) B(:, o)).
-template <int BN, bool FLIP, bool ONE_ROW, class Epi>
+// Forward / data gradient: epi(m, o, sum A(m, :) B(:, o)), A read through the input policy In.
+template <int BN, bool FLIP, bool ONE_ROW, class Epi, class In = PlainIn>
 __global__ void __launch_bounds__(CT_THREADS)
-conv_fwd_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, ConvGeom g, Epi epi) {
+conv_fwd_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, ConvGeom g, Epi epi, In in) {
+  static_assert(!In::ON || (!FLIP && !ONE_ROW && !Epi::GATED), "the input policy reads a forward 2-D window");
   constexpr int TILE_COLS = Epi::GATED ? BN / 2 : BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -197,7 +251,8 @@ conv_fwd_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, Con
   const int arow = tid >> 1, ahalf = tid & 1;
   const int64_t am = m0 + arow;
   const bool arow_ok = am < g.M;
-  const Pix ap = ONE_ROW ? row_pix(g, am, arow_ok ? (int)(am % g.W) : 0) : conv_pix<false>(g, arow_ok ? am : 0);
+  Pix ap = ONE_ROW ? row_pix(g, am, arow_ok ? (int)(am % g.W) : 0) : conv_pix<false>(g, arow_ok ? am : 0);
+  if constexpr (In::ON) in.origin(ap);
 
   auto gather = [&](int kb, uint8_t* st) {
     const int gk0 = kb * CT_BK + ahalf * 16;
@@ -207,15 +262,27 @@ conv_fwd_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, Con
         const int gk = gk0 + 4 * j;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         int64_t off;
-        if (arow_ok && gk < g.Kd && conv_a_at<ONE_ROW>(g, ap, gk, off))
+        if (arow_ok && gk < g.Kd && conv_a_at<ONE_ROW>(g, ap, gk, off)) {
           v = __ldg(reinterpret_cast<const float4*>(x + off));
+          if constexpr (In::ON) {
+            const int c = gk % g.C;   // C % 4 == 0: the 4 channels share a tap
+            v = make_float4(in.apply(v.x, c), in.apply(v.y, c + 1), in.apply(v.z, c + 2), in.apply(v.w, c + 3));
+          }
+        }
         sw128_store4(st, arow, ahalf * 4 + j, v);
       }
     } else {
 #pragma unroll 4
       for (int j = 0; j < 16; ++j) {
         const int gk = gk0 + j;
-        sw128_store1(st, arow, ahalf * 16 + j, (arow_ok && gk < g.Kd) ? conv_a<ONE_ROW>(x, g, ap, gk) : 0.f);
+        float v = 0.f;
+        if constexpr (In::ON) {
+          int64_t off;
+          if (arow_ok && gk < g.Kd && conv_a_at<ONE_ROW>(g, ap, gk, off)) v = in.apply(__ldg(x + off), gk % g.C);
+        } else {
+          v = (arow_ok && gk < g.Kd) ? conv_a<ONE_ROW>(x, g, ap, gk) : 0.f;
+        }
+        sw128_store1(st, arow, ahalf * 16 + j, v);
       }
     }
     uint8_t* bt = st + CT_A_BYTES;
@@ -431,9 +498,10 @@ conv_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, 
 // ------------------------------------------------------------------------------------------------------------
 constexpr int CS_BM = 64, CS_BN = 64, CS_TM = 4, CS_TN = 4;
 
-template <bool FLIP, bool ONE_ROW, class Epi>
+template <bool FLIP, bool ONE_ROW, class Epi, class In = PlainIn>
 __global__ void __launch_bounds__(SIMT_THREADS)
-conv_fwd_simt_kernel(const float* __restrict__ x, const float* __restrict__ w, ConvGeom g, Epi epi) {
+conv_fwd_simt_kernel(const float* __restrict__ x, const float* __restrict__ w, ConvGeom g, Epi epi, In in) {
+  static_assert(!In::ON || (!FLIP && !ONE_ROW && !Epi::GATED), "the input policy reads a forward 2-D window");
   constexpr int A_LOADS = (CS_BM * SIMT_BK) / SIMT_THREADS;
   __shared__ SimtSmem<CS_BM, CS_BN, CS_TM, CS_TN> sm;
   const int64_t m0 = (int64_t)blockIdx.x * CS_BM;
@@ -457,8 +525,14 @@ conv_fwd_simt_kernel(const float* __restrict__ x, const float* __restrict__ w, C
       const int64_t gm = m0 + mm;
       const int gk = k0 + kk;
       float v = 0.f;
-      if (arow_x[i] >= 0 && gk < g.Kd)
+      if constexpr (In::ON) {
+        Pix p = conv_pix<false>(g, gm);
+        in.origin(p);
+        int64_t off;
+        if (arow_x[i] >= 0 && gk < g.Kd && conv_a_at<false>(g, p, gk, off)) v = in.apply(__ldg(x + off), gk % g.C);
+      } else if (arow_x[i] >= 0 && gk < g.Kd) {
         v = conv_a<ONE_ROW>(x, g, ONE_ROW ? row_pix(g, gm, arow_x[i]) : conv_pix<false>(g, gm), gk);
+      }
       sm.a[kk][mm] = v;
     }
 #pragma unroll
@@ -594,9 +668,9 @@ static inline unsigned grid_for(int64_t total) {
 }
 
 // Forward / data-gradient launch on the engine `backend` selects, like nm_gemm's.
-template <int BN, bool FLIP, bool ONE_ROW, class Epi>
+template <int BN, bool FLIP, bool ONE_ROW, class Epi, class In = PlainIn>
 static int conv_fwd_launch(const float* x, const float* w, const ConvGeom& g, const Epi& epi, int backend,
-                           cudaStream_t s, const char* name) {
+                           cudaStream_t s, const char* name, const In& in = In{}) {
   // pixel tiles along x (up to 2^31 - 1 of them), output-column tiles along y
   const int64_t cols = epi.cols(g);
   if (backend == NM_GEMM_SIMT) {
@@ -604,7 +678,7 @@ static int conv_fwd_launch(const float* x, const float* w, const ConvGeom& g, co
     NM_REQUIRE(ceil_div(g.M, CS_BM) <= 0x7fffffffLL && ceil_div(cols, tile_cols) <= 65535, NM_E_UNSUPPORTED,
                "%s: grid too large", name);
     dim3 grid((unsigned)ceil_div(g.M, CS_BM), (unsigned)ceil_div(cols, tile_cols));
-    conv_fwd_simt_kernel<FLIP, ONE_ROW, Epi><<<grid, SIMT_THREADS, 0, s>>>(x, w, g, epi);
+    conv_fwd_simt_kernel<FLIP, ONE_ROW, Epi, In><<<grid, SIMT_THREADS, 0, s>>>(x, w, g, epi, in);
     NM_LAUNCH_CHECK(name);
     return NM_OK;
   }
@@ -614,12 +688,12 @@ static int conv_fwd_launch(const float* x, const float* w, const ConvGeom& g, co
              "%s: grid too large", name);
   static bool attr = false;
   if (!attr) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(conv_fwd_tc_kernel<BN, FLIP, ONE_ROW, Epi>,
+    NM_CUDA_TRY(cudaFuncSetAttribute(conv_fwd_tc_kernel<BN, FLIP, ONE_ROW, Epi, In>,
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, ct_smem<BN>()));
     attr = true;
   }
   dim3 grid((unsigned)ceil_div(g.M, CT_BM), (unsigned)ceil_div(cols, tile_cols));
-  conv_fwd_tc_kernel<BN, FLIP, ONE_ROW, Epi><<<grid, CT_THREADS, ct_smem<BN>(), s>>>(x, w, g, epi);
+  conv_fwd_tc_kernel<BN, FLIP, ONE_ROW, Epi, In><<<grid, CT_THREADS, ct_smem<BN>(), s>>>(x, w, g, epi, in);
   NM_LAUNCH_CHECK(name);
   return NM_OK;
 }

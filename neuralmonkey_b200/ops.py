@@ -1436,6 +1436,43 @@ def maxpool2x2(x: torch.Tensor) -> torch.Tensor:
     return y
 
 
+def conv2d_bn_fwd(x: torch.Tensor, w: torch.Tensor, stride: int = 1, pads: Tuple[int, int] = (0, 0),
+                  in_scale: Optional[torch.Tensor] = None, in_shift: Optional[torch.Tensor] = None,
+                  out_scale: Optional[torch.Tensor] = None, out_shift: Optional[torch.Tensor] = None,
+                  bias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None, res_stride: int = 1,
+                  act: Optional[str] = None) -> torch.Tensor:
+    """One frozen ResNet-v2 convolution (nm_conv2d_bn_fwd), forward only: NHWC x, HWIO w [k,k,Cin,Cout], `pads`
+    (before, after) on both axes, then
+        y = act(z + res[:, ::res_stride, ::res_stride]),  z = conv(A, w) * out_scale + out_shift  or  conv(A, w) + bias,
+    A = relu(x * in_scale + in_shift) (0 in the padding) when in_scale is given, else x.  The exact fp32 kernels
+    under the 'simt' GEMM backend, wgmma with TF32 operands otherwise."""
+    if act not in (None, "relu"):
+        raise ValueError("conv2d_bn_fwd: act must be None or 'relu'")
+    n, h, wd, cin = x.shape
+    k, cout = w.shape[0], w.shape[3]
+    if tuple(w.shape[1:3]) != (k, cin):
+        raise ValueError("conv2d_bn_fwd: filter {} does not fit input {}".format(tuple(w.shape), tuple(x.shape)))
+    pt, pb = pads
+    ho, wo = (h + pt + pb - k) // stride + 1, (wd + pt + pb - k) // stride + 1
+
+    def vec(t):
+        return None if t is None else _f32(t.detach()).contiguous()
+
+    x, w = _f32(x.detach()).contiguous(), _f32(w.detach()).contiguous()
+    res_h = res_w = 0
+    if res is not None:
+        res = vec(res)
+        if res.shape[0] != n or res.shape[3] != cout:
+            raise ValueError("conv2d_bn_fwd: residual {} does not fit output {}".format(
+                tuple(res.shape), (n, ho, wo, cout)))
+        res_h, res_w = res.shape[1], res.shape[2]
+    vecs = [vec(t) for t in (in_scale, in_shift, out_scale, out_shift, bias)]   # alive until the call returns
+    y = torch.empty(n, max(ho, 0), max(wo, 0), cout, device=x.device, dtype=torch.float32)
+    call("nm_conv2d_bn_fwd", ptr(x), ptr(w), *[ptr(t) for t in vecs], ptr(res), res_h, res_w, res_stride, ptr(y), n,
+         h, wd, cin, cout, k, stride, pt, pb, pt, pb, lib.NM_ACT[act], _conv_backend(), lib.stream())
+    return y
+
+
 # ---------------------------------------------------------------------------
 # K12b trainable CNN layers (encoders/cnn_encoder.py): convolution, batch normalization, pooling
 # ---------------------------------------------------------------------------
