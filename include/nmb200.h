@@ -211,10 +211,12 @@ int nm_bahdanau_fwd(const float* keys, const float* values, const float* mask,
 /* Backward.  dkeys [B,Tx,A], dvalues [B,Tx,C], dqproj [B,NQ,A] are overwritten;
  * dv [A] and dbias [1] are accumulated into.  Gradient reaches the energies of
  * masked positions too (the softmax runs before the mask), as in the reference.
- * de_work is scratch of B*NQ*Tx floats. */
+ * de_in [B,NQ,Tx] (may be NULL = none) is a gradient of a loss on the energies
+ * themselves (K21); it is added to the energy gradient derived from dctx before
+ * that reaches keys, qproj, v and bias.  de_work is scratch of B*NQ*Tx floats. */
 int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask,
                     const float* qproj, const float* v, const float* energies,
-                    const float* weights, const float* dctx, float* dkeys,
+                    const float* weights, const float* dctx, const float* de_in, float* dkeys,
                     float* dvalues, float* dqproj, float* dv, float* dbias,
                     float* de_work, int64_t B, int64_t Tx, int64_t NQ, int64_t A,
                     int64_t C, void* stream);
@@ -829,6 +831,20 @@ int nm_speech_features(const double* signal, int64_t samples, const double* wind
                        int64_t out_stride, void* stream);
 int nm_speech_deltas(double* out, int64_t frames, int64_t width, int64_t out_stride, int64_t block, int64_t window,
                      void* stream);
+
+/* ---- K21: supervised attention: cross-entropy of attention energies against word alignments ------------------
+ * Replaces the training loss of decoders/word_alignment_decoder.py:100-108, softmax_cross_entropy_with_logits over
+ * the K4 energies (all Tx positions, padding included) times the decoder's training padding, summed:
+ *     loss = sum_{b,q} pad[b,q] * sum_t target[b,q,t] * (lse_t energies[b,q,t] - energies[b,q,t])
+ * energies, target [B,NQ,Tx], pad [B,NQ] fp32 (all device).
+ * nm_alignment_xent_fwd: loss [1]; workspace holds B*NQ floats (the row losses), which one CTA sums in a fixed
+ *   order: repeat calls give identical bits.
+ * nm_alignment_xent_bwd: de_out [B,NQ,Tx] = grad_loss[0] * pad * (softmax_t(energies) * sum_t target - target),
+ *   overwritten; grad_loss [1] is a device scalar.  de_out is what nm_bahdanau_bwd takes as de_in. */
+int nm_alignment_xent_fwd(const float* energies, const float* target, const float* pad, float* loss,
+                          float* workspace, int64_t B, int64_t NQ, int64_t Tx, void* stream);
+int nm_alignment_xent_bwd(const float* energies, const float* target, const float* pad, const float* grad_loss,
+                          float* de_out, int64_t B, int64_t NQ, int64_t Tx, void* stream);
 
 #ifdef __cplusplus
 }

@@ -74,16 +74,23 @@ class Attention(BaseAttention):
         """U_a . states, [batch, time, state_size] (feed_forward.py:111-118)."""
         return ops.linear(self.attention_states, self.var("attn_key_projection"))
 
-    def attention_sequence(self, queries: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        """All query steps at once: queries [batch, NQ, query_size] ->
-        (contexts [batch, NQ, ctx], weights [batch, NQ, time])."""
+    def _operands(self, queries: torch.Tensor):
         y = ops.linear(queries, self.var("Attention/attn_query_projection"),
                        self.var("attn_projection_bias"))
         keys, values, mask = self.hidden_features, self.attention_states, self.attention_mask
         if queries.shape[0] != keys.shape[0]:
             keys, values, mask = self._beam_tiled(queries.shape[0])
-        return ops.bahdanau_attention(keys, values, mask, y, self.var("attn_similarity_v"),
-                                      self.var("attn_bias"))
+        return keys, values, mask, y, self.var("attn_similarity_v"), self.var("attn_bias")
+
+    def attention_sequence(self, queries: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """All query steps at once: queries [batch, NQ, query_size] ->
+        (contexts [batch, NQ, ctx], weights [batch, NQ, time])."""
+        return ops.bahdanau_attention(*self._operands(queries))
+
+    def attention_sequence_energies(self, queries: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """`attention_sequence` that also returns the pre-softmax energies [batch, NQ, time] of the same evaluation,
+        differentiable (the reference's attention logits, feed_forward.py:136-137)."""
+        return ops.bahdanau_attention_energies(*self._operands(queries))
 
     def _beam_tiled(self, rows: int):
         """Keys / values / mask repeated beam-minor for a BeamSearchDecoder parent.  The

@@ -110,13 +110,15 @@ bahdanau_fwd_kernel(const float* __restrict__ keys, const float* __restrict__ va
   }
 }
 
-// Backward A: de[b,q,t] from dctx.  grid (nch, B) as the forward.
+// Backward A: de[b,q,t] from dctx, plus de_in (a loss on the energies themselves) when given.  grid (nch, B) as
+// the forward.  DE_IN is whether de_in is given: without it the kernel is the plain dctx path.
 // dynamic smem: dcs[QMAX][C] (the chunk's dctx rows, zero beyond nq) | dws[QMAX][Tx]
+template <bool DE_IN>
 __global__ void __launch_bounds__(ATT_THREADS)
 bahdanau_bwd_energy_kernel(const float* __restrict__ values, const float* __restrict__ mask,
                            const float* __restrict__ energies, const float* __restrict__ weights,
-                           const float* __restrict__ dctx, float* __restrict__ de,
-                           float* __restrict__ dbias, int Tx, int NQ, int C) {
+                           const float* __restrict__ dctx, const float* __restrict__ de_in,
+                           float* __restrict__ de, float* __restrict__ dbias, int Tx, int NQ, int C) {
   extern __shared__ float smem[];
   float* dcs = smem;
   float* dws = dcs + ATT_QMAX * C;
@@ -185,7 +187,8 @@ bahdanau_bwd_energy_kernel(const float* __restrict__ values, const float* __rest
     pdp = warp_sum(pdp);
     for (int t = lane; t < Tx; t += 32) {
       const float p = expf(er[t] - mx) / s;
-      const float g = p * (dwr[t] - pdp);
+      float g = p * (dwr[t] - pdp);
+      if (DE_IN) g += de_in[row + t];
       de[row + t] = g;
       dbias_local += g;
     }
@@ -326,7 +329,8 @@ int nm_bahdanau_fwd(const float* keys, const float* values, const float* mask, c
 
 int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask, const float* qproj,
                     const float* v, const float* energies, const float* weights, const float* dctx,
-                    float* dkeys, float* dvalues, float* dqproj, float* dv, float* dbias, float* de_work,
+                    const float* de_in, float* dkeys, float* dvalues, float* dqproj, float* dv, float* dbias,
+                    float* de_work,
                     int64_t B, int64_t Tx, int64_t NQ, int64_t A, int64_t C, void* stream) {
   NM_REQUIRE(keys && values && qproj && v && energies && weights && dctx && dkeys && dvalues &&
                  dqproj && dv && dbias && de_work,
@@ -342,7 +346,9 @@ int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask, c
              (long long)NQ, (long long)Tx, (long long)C, smem_a, smem_b, smem_c);
   static bool attr_set = false;
   if (!attr_set) {
-    NM_CUDA_TRY(cudaFuncSetAttribute(bahdanau_bwd_energy_kernel,
+    NM_CUDA_TRY(cudaFuncSetAttribute(bahdanau_bwd_energy_kernel<false>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM_LIMIT));
+    NM_CUDA_TRY(cudaFuncSetAttribute(bahdanau_bwd_energy_kernel<true>,
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM_LIMIT));
     NM_CUDA_TRY(cudaFuncSetAttribute(bahdanau_bwd_keys_kernel,
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM_LIMIT));
@@ -351,8 +357,13 @@ int nm_bahdanau_bwd(const float* keys, const float* values, const float* mask, c
     attr_set = true;
   }
   dim3 grid_a((unsigned)att_chunks(B, NQ), (unsigned)B);
-  bahdanau_bwd_energy_kernel<<<grid_a, ATT_THREADS, smem_a, s>>>(values, mask, energies, weights, dctx,
-                                                                de_work, dbias, (int)Tx, (int)NQ, (int)C);
+  if (de_in)
+    bahdanau_bwd_energy_kernel<true><<<grid_a, ATT_THREADS, smem_a, s>>>(values, mask, energies, weights, dctx, de_in,
+                                                                        de_work, dbias, (int)Tx, (int)NQ, (int)C);
+  else
+    bahdanau_bwd_energy_kernel<false><<<grid_a, ATT_THREADS, smem_a, s>>>(values, mask, energies, weights, dctx,
+                                                                         nullptr, de_work, dbias, (int)Tx, (int)NQ,
+                                                                         (int)C);
   NM_LAUNCH_CHECK("nm_bahdanau_bwd(energy)");
   dim3 grid_b((unsigned)ceil_div(A, ATT_ACH), (unsigned)B);
   bahdanau_bwd_keys_kernel<<<grid_b, ATT_ACH, smem_b, s>>>(keys, qproj, v, de_work, dkeys, dqproj, dv,

@@ -21,6 +21,7 @@ from neuralmonkey_b200.typecheck import check_argument_types
 from neuralmonkey_b200 import ops, runtime
 from neuralmonkey_b200.attention.base_attention import BaseAttention
 from neuralmonkey_b200.attention.coverage import CoverageAttention
+from neuralmonkey_b200.attention.feed_forward import Attention
 from neuralmonkey_b200.decoders.autoregressive import AutoregressiveDecoder, LoopState
 from neuralmonkey_b200.decoders.encoder_projection import (
     EncoderProjection, concat_encoder_projection, empty_initial_state, linear_encoder_projection)
@@ -85,6 +86,7 @@ class Decoder(AutoregressiveDecoder):
             raise NotImplementedError("attention_on_input=True fails in the reference while the graph is "
                                       "built (decoders/decoder.py:273); it is not supported here either")
         self._stepwise = self._rnn_cell_str != "GRU" or conditional_gru
+        self._supervised_attentions = []      # type: List[BaseAttention]
         for att in self.attentions:
             if hasattr(att, "set_query_size"):
                 att.set_query_size(self.rnn_size)
@@ -188,14 +190,43 @@ class Decoder(AutoregressiveDecoder):
             init = init.unsqueeze(0).expand(self.batch_size, -1).contiguous()
         return init
 
-    @staticmethod
-    def _attend_sequence(att, queries, prev_outputs, inputs):
-        """att.attention_sequence over queries [B, NQ, rnn]; attentions that declare `wants_sentinel_inputs`
-        (attention.combination) also get each query step's previous cell output and embedded input
-        [B, NQ, .], which `next_state` hands to `attention()` at run time."""
+    def supervise_attention(self, encoder: Stateful) -> Attention:
+        """The attention of this decoder over `encoder`, from now on evaluated so that its training pass also
+        yields the attention energies (`train_attention_energies`) for a loss on them (WordAlignmentDecoder).
+        Only the Bahdanau `attention.Attention` has such energies here; any other class is refused."""
+        def over(att) -> bool:
+            return any(getattr(att, name, None) is encoder for name in ("encoder", "keys_encoder", "values_encoder"))
+        found = [att for att in self.attentions if over(att)]
+        if not found:
+            raise ValueError("Decoder '{}' has no attention over encoder '{}'".format(
+                self.name, getattr(encoder, "name", encoder)))
+        att = found[0]
+        if type(att) is not Attention:      # pylint: disable=unidiomatic-typecheck
+            raise ValueError("Attention '{}' of decoder '{}' is a {}: supervising the attention needs the Bahdanau "
+                             "attention.Attention, whose energies the loss is defined on".format(
+                                 att.name, self.name, type(att).__name__))
+        if att not in self._supervised_attentions:
+            self._supervised_attentions.append(att)
+        return att
+
+    def train_attention_energies(self, att: Attention) -> torch.Tensor:
+        """[batch, steps, time] pre-softmax energies of `att` (see `supervise_attention`) in this batch's training
+        pass: the same attention evaluation as the decoder's own, so one backward call reaches both."""
+        energies = self._train_pass[3][self.attentions.index(att)]
+        if energies is None:
+            raise ValueError("Attention '{}' is not supervised by decoder '{}'".format(att.name, self.name))
+        return energies
+
+    def _attend_sequence(self, att, queries, prev_outputs, inputs):
+        """(contexts, weights, energies) of att over queries [B, NQ, rnn].  Attentions that declare
+        `wants_sentinel_inputs` (attention.combination) also get each query step's previous cell output and embedded
+        input [B, NQ, .], which `next_state` hands to `attention()` at run time.  `energies` [B, NQ, time] are
+        differentiable for a supervised attention (`supervise_attention`), None for the others."""
         if getattr(att, "wants_sentinel_inputs", False):
-            return att.attention_sequence(queries, prev_outputs, inputs)
-        return att.attention_sequence(queries)
+            return att.attention_sequence(queries, prev_outputs, inputs) + (None,)
+        if att in self._supervised_attentions:
+            return att.attention_sequence_energies(queries)
+        return att.attention_sequence(queries) + (None,)
 
     def _step_attend(self, prev_output, rnn_input, coverage):
         """`attend(att, query)` of one teacher-forced or differentiable step: prev_output is what the step
@@ -206,9 +237,9 @@ class Decoder(AutoregressiveDecoder):
         def attend(att, query):
             if isinstance(att, CoverageAttention):
                 ctx, w, coverage[id(att)] = att.coverage_scan(query.unsqueeze(1), coverage.get(id(att)))
-                return ctx[:, 0], w
-            ctx, w = self._attend_sequence(att, query.unsqueeze(1), prev_h.unsqueeze(1), rnn_input.unsqueeze(1))
-            return ctx[:, 0], w
+                return ctx[:, 0], w, None
+            ctx, w, e = self._attend_sequence(att, query.unsqueeze(1), prev_h.unsqueeze(1), rnn_input.unsqueeze(1))
+            return ctx[:, 0], w, e
         return attend
 
     # -- variants: one step of decoder.py:279-358 with the context inside the recurrence ---------
@@ -247,18 +278,21 @@ class Decoder(AutoregressiveDecoder):
         prev = self.initial_state
         if self._rnn_cell_str == "LSTM":
             prev = (prev, prev)
-        outputs, cells, weights, coverage = [], [], [[] for _ in self.attentions], {}
+        outputs, cells, coverage = [], [], {}
+        weights, energies = [[] for _ in self.attentions], [[] for _ in self.attentions]
         for t in range(fed.shape[1]):       # one query per sentence and step: NQ = 1
             out, prev, _ctx, attended = self._variant_step(emb[:, t], prev,
                                                            self._step_attend(prev, emb[:, t], coverage))
             outputs.append(out)
             cells.append(prev[1] if isinstance(prev, tuple) else prev)
-            for hist, (_c, w) in zip(weights, attended):
+            for hist, e_hist, (_c, w, e) in zip(weights, energies, attended):
                 hist.append(w)
+                e_hist.append(e)
         weights = [torch.cat(hist, dim=-2) for hist in weights]     # the query axis is the one before time
+        energies = [torch.cat(hist, dim=-2) if hist[0] is not None else None for hist in energies]
         for att, w in zip(self.attentions, weights):
             att.record_weights("{}_train".format(self.name), w)
-        return torch.stack(outputs, 1), torch.stack(cells, 1), weights
+        return torch.stack(outputs, 1), torch.stack(cells, 1), weights, energies
 
     # -- training: all steps at once ------------------------------------------------------
     @tensor
@@ -276,15 +310,16 @@ class Decoder(AutoregressiveDecoder):
         prev_outputs = None
         if any(getattr(att, "wants_sentinel_inputs", False) for att in self.attentions):
             prev_outputs = torch.cat([self.initial_state.unsqueeze(1), dropped[:, :-1]], 1)
-        contexts, weights = [], []
+        contexts, weights, energies = [], [], []
         for att in self.attentions:
-            ctx, w = self._attend_sequence(att, raw, prev_outputs, emb)   # queries = cell outputs BEFORE dropout
+            ctx, w, e = self._attend_sequence(att, raw, prev_outputs, emb)   # queries = cell outputs BEFORE dropout
             contexts.append(dropout(ctx, self.dropout_keep_prob, self.train_mode))
             weights.append(w)
+            energies.append(e)
         out = self.output_projection(self, dropped, emb, contexts, self.train_mode)  # [B,T,O]
         for att, w in zip(self.attentions, weights):
             att.record_weights("{}_train".format(self.name), w)
-        return out, dropped, weights
+        return out, dropped, weights, energies
 
     @property
     def _train_states_bm(self) -> torch.Tensor:

@@ -658,16 +658,18 @@ class _Bahdanau(torch.autograd.Function):
         ctx.save_for_backward(keys, values, mask_c, qproj, v, energies, weights)
         ctx.sinks = (_sink(v), _sink(bias))
         ctx.mark_non_differentiable(weights)
-        return ctxv, weights
+        ctx.set_materialize_grads(False)
+        return ctxv, weights, energies
 
     @staticmethod
-    def backward(ctx, dctx, _dweights):
+    def backward(ctx, dctx, _dweights, denergies):
         keys, values, mask, qproj, v, energies, weights = ctx.saved_tensors
         bsz, tx, a = keys.shape
         c = values.size(2)
         nq = qproj.size(1)
         dev = keys.device
-        dctx = dctx.contiguous()
+        dctx = dctx.contiguous() if dctx is not None else torch.zeros(bsz, nq, c, device=dev, dtype=torch.float32)
+        denergies = denergies.contiguous() if denergies is not None else None
         dkeys = torch.empty_like(keys)
         dvalues = torch.empty_like(values)
         dq = torch.empty_like(qproj)
@@ -676,7 +678,7 @@ class _Bahdanau(torch.autograd.Function):
         db = sb if sb is not None else torch.zeros(1, device=dev, dtype=torch.float32)
         work = torch.empty(bsz * nq * tx, device=dev, dtype=torch.float32)
         call("nm_bahdanau_bwd", ptr(keys), ptr(values), ptr(mask), ptr(qproj), ptr(v), ptr(energies),
-             ptr(weights), ptr(dctx), ptr(dkeys), ptr(dvalues), ptr(dq), ptr(dv), ptr(db), ptr(work),
+             ptr(weights), ptr(dctx), ptr(denergies), ptr(dkeys), ptr(dvalues), ptr(dq), ptr(dv), ptr(db), ptr(work),
              bsz, tx, nq, a, c, lib.stream())
         return (dkeys, dvalues, None, dq, None if sv is not None else dv,
                 None if sb is not None else db)
@@ -689,7 +691,58 @@ def bahdanau_attention(keys: torch.Tensor, values: torch.Tensor, mask: Optional[
 
     keys [B,Tx,A], values [B,Tx,C], mask [B,Tx] or None, qproj [B,NQ,A], v [A], bias [1].
     Returns (contexts [B,NQ,C], weights [B,NQ,Tx])."""
+    ctxv, weights, _energies = _Bahdanau.apply(keys, values, mask, qproj, v, bias)
+    return ctxv, weights
+
+
+def bahdanau_attention_energies(keys: torch.Tensor, values: torch.Tensor, mask: Optional[torch.Tensor],
+                                qproj: torch.Tensor, v: torch.Tensor,
+                                bias: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """`bahdanau_attention` that also returns the pre-softmax energies e [B,NQ,Tx] of the same evaluation, as a
+    differentiable output: a loss on them (`alignment_xent`) reaches keys, qproj, v and bias through the same
+    nm_bahdanau_bwd call as the gradient of the contexts.  Returns (contexts, weights, energies)."""
     return _Bahdanau.apply(keys, values, mask, qproj, v, bias)
+
+
+# ---------------------------------------------------------------------------
+# K21 supervised attention (decoders.word_alignment_decoder)
+# ---------------------------------------------------------------------------
+class _AlignmentXent(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, energies, target, pad):
+        bsz, nq, tx = energies.shape
+        energies, target, pad = energies.contiguous(), target.contiguous(), pad.contiguous()
+        dev = energies.device
+        loss = torch.empty((), device=dev, dtype=torch.float32)
+        work = torch.empty(bsz * nq, device=dev, dtype=torch.float32)
+        call("nm_alignment_xent_fwd", ptr(energies), ptr(target), ptr(pad), ptr(loss), ptr(work), bsz, nq, tx,
+             lib.stream())
+        ctx.save_for_backward(energies, target, pad)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        energies, target, pad = ctx.saved_tensors
+        bsz, nq, tx = energies.shape
+        de = torch.empty_like(energies)
+        call("nm_alignment_xent_bwd", ptr(energies), ptr(target), ptr(pad), ptr(dloss.contiguous()),
+             ptr(de), bsz, nq, tx, lib.stream())
+        return de, None, None
+
+
+def alignment_xent(energies: torch.Tensor, target: torch.Tensor, pad: torch.Tensor) -> torch.Tensor:
+    """The training loss of WordAlignmentDecoder (decoders/word_alignment_decoder.py:100-108): a scalar
+
+        sum_{b,q} pad[b,q] * sum_t target[b,q,t] * (logsumexp_t energies[b,q,t] - energies[b,q,t]),
+
+    softmax cross-entropy over all Tx positions.  energies, target [B,NQ,Tx], pad [B,NQ]; differentiable in the
+    energies only.  The sum is taken in a fixed order: repeat calls give the same bits."""
+    for t in (energies, target, pad):
+        _f32(t)
+    if target.shape != energies.shape or pad.shape != energies.shape[:2]:
+        raise ValueError("alignment_xent: energies {}, target {}, pad {}".format(
+            tuple(energies.shape), tuple(target.shape), tuple(pad.shape)))
+    return _AlignmentXent.apply(energies, target, pad)
 
 
 # ---------------------------------------------------------------------------

@@ -61,6 +61,11 @@ class GenericTrainer(GraphExecutor, Feedable):
                 # their loop length and rewards depend on the data: a captured step could not replay them
                 raise ValueError("use_cuda_graph=True cannot capture the step of objective(s) {}: their decoding "
                                  "loops stop and score on the host".format(", ".join(eager)))
+            extra = [obj.name for obj in objectives if not getattr(obj.decoder, "graph_capturable", True)]
+            if extra:
+                raise ValueError("use_cuda_graph=True cannot capture the step of objective(s) {}: a captured step "
+                                 "computes one token-mean cross-entropy objective, and these add a loss of "
+                                 "their own".format(", ".join(extra)))
 
     @property
     def global_step(self) -> int:

@@ -89,7 +89,7 @@ def main():
 
         def bwd():
             lib.call("nm_bahdanau_bwd", p(keys), p(values), p(mask), p(qproj), p(v), p(energies), p(weights),
-                     p(dctx), p(dkeys), p(dvalues), p(dq), p(dv), p(db), p(work), b, tx, nq, a, c, st)
+                     p(dctx), None, p(dkeys), p(dvalues), p(dq), p(dv), p(db), p(work), b, tx, nq, a, c, st)
 
         t_f, t_b = time_calls(fwd, args.iters), time_calls(bwd, args.iters)
         floor = b * nq * tx * a / (sms * SFU_PER_CLOCK_PER_SM * max_mhz * 1e3)   # ms, 1 SFU op per element
