@@ -846,6 +846,38 @@ int nm_alignment_xent_fwd(const float* energies, const float* target, const floa
 int nm_alignment_xent_bwd(const float* energies, const float* target, const float* pad, const float* grad_loss,
                           float* de_out, int64_t B, int64_t NQ, int64_t Tx, void* stream);
 
+/* ---- K22: the character-level sentence encoder (encoders/sentence_cnn_encoder.py, nn/highway.py; csrc/
+ * sentence_cnn.cu on the implicit-GEMM kernels of csrc/conv_igemm.cuh: a 1 x k window over [B, 1, T, Cin]) -----
+ * x [B,T,Cin], w [k,Cin,Cout], bias [Cout], fp32, row-major; M = B*T.
+ *   y = act(conv1d(x, w) + bias)   tf.nn.conv1d at stride 1 with SAME padding: (k-1)/2 zeros before each sequence,
+ *                                  the rest after; positions inside [0,T) always take part, padded batch positions
+ *                                  included.  act is NM_ACT_NONE or NM_ACT_RELU.
+ * Any B, T (T < k and T = 1 included), Cin, Cout and k.  backend: NM_GEMM_SIMT = exact fp32 on the CUDA cores,
+ * NM_GEMM_AUTO / NM_GEMM_TC = wgmma with TF32 operands.  Implicit GEMMs: no patch matrix.
+ * nm_conv1d_fwd: y [B,T,Cout]; bias may be NULL.
+ * nm_conv1d_dgrad: dx [B,T,Cin] = conv1d of dy [B,T,Cout] (the gradient of the pre-activation) with w's taps
+ *   reversed and channel axes swapped; dx must not alias dy.
+ * nm_conv1d_wgrad: dw [k,Cin,Cout] += sum over positions of patch(x)^T dy, db [Cout] += sum dy (db may be NULL).
+ *   The position sum is split over CTAs into `workspace` (>= (k*Cin+1)*Cout floats; more lets it split further)
+ *   and the partials are added in a fixed order: two calls give identical bits.
+ * nm_conv1d_wgrad_workspace: the workspace (floats) at which nm_conv1d_wgrad splits as far as it wants to for that
+ *   shape and backend, or -1 for invalid sizes.
+ * nm_highway_fwd: the highway gate over the n elements of the two dense products' outputs zh = x W_H + b_H and
+ *   zt = x W_T + b_T and of x:  y = relu(zh) * sigmoid(zt) + x * (1 - sigmoid(zt)).
+ * nm_highway_bwd: dzh = dy t [zh > 0], dzt = dy (relu(zh) - x) t (1 - t), dx = dy (1 - t) with t = sigmoid(zt):
+ *   the gradients of both products' outputs and the carry term of dx.  Element by element: repeat calls give
+ *   identical bits. */
+int nm_conv1d_fwd(const float* x, const float* w, const float* bias, float* y, int64_t B, int64_t T, int64_t Cin,
+                  int64_t Cout, int64_t k, int act, int backend, void* stream);
+int nm_conv1d_dgrad(const float* dy, const float* w, float* dx, int64_t B, int64_t T, int64_t Cin, int64_t Cout,
+                    int64_t k, int backend, void* stream);
+int64_t nm_conv1d_wgrad_workspace(int64_t B, int64_t T, int64_t Cin, int64_t Cout, int64_t k, int backend);
+int nm_conv1d_wgrad(const float* x, const float* dy, float* dw, float* db, float* workspace, int64_t workspace_floats,
+                    int64_t B, int64_t T, int64_t Cin, int64_t Cout, int64_t k, int backend, void* stream);
+int nm_highway_fwd(const float* zh, const float* zt, const float* x, float* y, int64_t n, void* stream);
+int nm_highway_bwd(const float* dy, const float* zh, const float* zt, const float* x, float* dzh, float* dzt,
+                   float* dx, int64_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

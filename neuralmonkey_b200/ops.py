@@ -1669,6 +1669,103 @@ def conv1d_glu_residual(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> to
     return _Conv1dGluResidual.apply(x, w, b)
 
 
+# ---------------------------------------------------------------------------
+# K22 character-level sentence encoder (encoders/sentence_cnn_encoder.py): the one-row convolution, the highway gate
+# ---------------------------------------------------------------------------
+def conv1d_wgrad_workspace(bsz, t, cin, cout, k, backend) -> int:
+    want = int(lib.load().nm_conv1d_wgrad_workspace(bsz, t, cin, cout, k, backend))
+    if want < 0:
+        raise ValueError("conv1d: bad sizes {}".format((bsz, t, cin, cout, k)))
+    return max((k * cin + 1) * cout, min(_WGRAD_WS_FLOATS, want))
+
+
+class _Conv1d(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b, act):
+        bsz, t, cin = x.shape
+        k, cout = w.shape[0], w.shape[2]
+        if w.shape[1] != cin or (b is not None and tuple(b.shape) != (cout,)):
+            raise ValueError("conv1d: filter {} / bias {} do not fit input {}".format(
+                tuple(w.shape), None if b is None else tuple(b.shape), tuple(x.shape)))
+        x = _f32(x).contiguous()
+        w = _f32(w).contiguous()
+        y = torch.empty(bsz, t, cout, device=x.device, dtype=torch.float32)
+        backend = _conv_backend()
+        call("nm_conv1d_fwd", ptr(x), ptr(w), ptr(b), ptr(y), bsz, t, cin, cout, k, lib.NM_ACT[act], backend,
+             lib.stream())
+        ctx.save_for_backward(x, w, y if act is not None else None)
+        ctx.geom = (bsz, t, cin, cout, k, backend, act)
+        ctx.sinks = (_sink(w), _sink(b) if b is not None else None)
+        ctx.has_bias = b is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, y = ctx.saved_tensors
+        bsz, t, cin, cout, k, backend, act = ctx.geom
+        dy = _f32(dy).contiguous()
+        if act is not None:
+            dpre = torch.empty_like(dy)
+            call("nm_act_bwd", ptr(y), ptr(dy), ptr(dpre), dy.numel(), lib.NM_ACT[act], lib.stream())
+            dy = dpre
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            call("nm_conv1d_dgrad", ptr(dy), ptr(w), ptr(dx), bsz, t, cin, cout, k, backend, lib.stream())
+        w_sink, b_sink = ctx.sinks
+        if not (ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2])):
+            return dx, None, None, None
+        dw = w_sink if w_sink is not None else torch.zeros_like(w)
+        db = None
+        if ctx.has_bias:
+            db = b_sink if b_sink is not None else torch.zeros(cout, device=x.device, dtype=torch.float32)
+        ws = torch.empty(conv1d_wgrad_workspace(bsz, t, cin, cout, k, backend), device=x.device, dtype=torch.float32)
+        call("nm_conv1d_wgrad", ptr(x), ptr(dy), ptr(dw), ptr(db), ptr(ws), ws.numel(), bsz, t, cin, cout, k, backend,
+             lib.stream())
+        return (dx, None if w_sink is not None else dw,
+                None if (b_sink is not None or not ctx.has_bias) else db, None)
+
+
+def conv1d(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], padding: str = "same",
+           act: Optional[str] = None) -> torch.Tensor:
+    """act(tf.nn.conv1d(x, w, 1, 'SAME') + b): x [B,T,Cin], w [k,Cin,Cout], b [Cout] or None, act None or 'relu'.
+    The one-row kernels keep the sequence length, so `padding` is 'same' only.  The exact fp32 kernels under the
+    'simt' GEMM backend, wgmma with TF32 operands otherwise."""
+    if padding != "same":
+        raise ValueError("conv1d: padding must be 'same', got {!r}".format(padding))
+    if act not in (None, "relu"):
+        raise ValueError("conv1d: act must be None or 'relu'")
+    return _Conv1d.apply(x, w, b, act)
+
+
+class _HighwayGate(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, zh, zt, x):
+        if zh.shape != x.shape or zt.shape != x.shape:
+            raise ValueError("highway_gate: shapes {}, {} and {} differ".format(
+                tuple(zh.shape), tuple(zt.shape), tuple(x.shape)))
+        zh, zt, x = (_f32(a).contiguous() for a in (zh, zt, x))
+        y = torch.empty_like(x)
+        call("nm_highway_fwd", ptr(zh), ptr(zt), ptr(x), ptr(y), x.numel(), lib.stream())
+        ctx.save_for_backward(zh, zt, x)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        zh, zt, x = ctx.saved_tensors
+        dy = _f32(dy).contiguous()
+        dzh, dzt, dx = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
+        call("nm_highway_bwd", ptr(dy), ptr(zh), ptr(zt), ptr(x), ptr(dzh), ptr(dzt), ptr(dx), x.numel(),
+             lib.stream())
+        return dzh, dzt, dx
+
+
+def highway_gate(zh: torch.Tensor, zt: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """relu(zh) * sigmoid(zt) + x * (1 - sigmoid(zt)) for the outputs zh, zt of a highway layer's two dense
+    products; the backward gives both products' output gradients and the carry term of dx."""
+    return _HighwayGate.apply(zh, zt, x)
+
+
 BN_WS_DOUBLES_PER_CHANNEL = 130     # NM_BN_WS_DOUBLES_PER_CHANNEL
 
 
