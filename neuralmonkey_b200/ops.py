@@ -1232,6 +1232,13 @@ class _MHADrop(torch.autograd.Function):
         return dq, dk, dv, None, None, None, None
 
 
+def _tma_operand(t: torch.Tensor) -> torch.Tensor:
+    """t contiguous and starting on a 16-byte boundary, as a tensor map addresses it: a copy when a view starts
+    elsewhere."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 class _MHATensorCore(torch.autograd.Function):
     """The attention core as batched wgmma products (csrc/mha_tc.cu): softmax and its backward in the GEMM
     epilogues, all (sentence, head) pairs in one launch per product.  TF32 operands."""
@@ -1240,7 +1247,7 @@ class _MHATensorCore(torch.autograd.Function):
     def forward(ctx, q, k, v, key_mask, causal, heads, drop_mask):
         bsz, tq, d = q.shape
         tk = k.size(1)
-        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        q, k, v = _tma_operand(q), _tma_operand(k), _tma_operand(v)
         mask_c = key_mask.contiguous() if key_mask is not None else None
         drop_c = drop_mask.to(torch.float32).contiguous() if drop_mask is not None else None
         tqp, tkp = (tq + 31) // 32 * 32, (tk + 31) // 32 * 32
@@ -1261,7 +1268,7 @@ class _MHATensorCore(torch.autograd.Function):
         causal, heads = ctx.cfg
         bsz, tq, d = q.shape
         tk = k.size(1)
-        dout = dout.contiguous()
+        dout = _tma_operand(dout)
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
         work = torch.empty_like(probs)
         call("nm_mha_tc_bwd", ptr(q), ptr(k), ptr(v), ptr(mask), int(causal), ptr(drop_c), ptr(probs),
